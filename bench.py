@@ -1,7 +1,7 @@
-"""Headline benchmark: forward images/sec of a tfimm classifier on N B200 GPUs (one node).
+"""Headline benchmark: forward images/sec of a tfimm classifier on N H100 GPUs (one node).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--model vit_base_patch16_224]
-                    [--batch 256] [--impl b200|reference]
+                    [--batch 256] [--impl b200|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one forward pass of the model over one synthetic batch (``--batch`` images per GPU,
@@ -10,6 +10,10 @@ prints ONE JSON line (see the task contract): whole-job images/sec with inputs r
 (``value``), the same through the public API from pinned host memory (``e2e``), the roofline of
 the dominant kernel family measured live with CUDA events, the CPU oracle timed beside it, and the
 SM clocks sampled during the timed region.
+
+``--dump-outputs DIR`` writes, for every timed model, the logits of the last timed step as
+``DIR/<model>.npy`` (float32, the whole [global batch, classes] array).  Inputs and weights are
+seeded, so two builds run with the same arguments can be compared output for output.
 
 ``--impl reference`` times the CPU stand-in for the reference (the torch-CPU oracle restatement;
 TensorFlow is not installed in this image, see BASELINE.md section 3) on the same config.
@@ -31,7 +35,7 @@ sys.path.insert(0, str(ROOT))
 METRIC = "images/sec fwd bs=256 224px"
 # the other BASELINE.json configs, timed after the headline model and reported under "extra"
 EXTRA_MODELS = ["convnext_base", "swin_base_patch4_window7_224", "efficientnet_b4"]
-# Algorithmic work per image (SURVEY.md 8d): GFLOP and op-level HBM MB in bf16
+# Algorithmic work per image (BASELINE.md section 2): GFLOP and op-level HBM MB in bf16
 WORK = {
     "vit_base_patch16_224": {"gflop": 35.13, "mb": 80.5, "bound": "tensor"},
     "vit_tiny_patch16_224": {"gflop": 2.51, "mb": 20.3, "bound": "tensor"},
@@ -47,7 +51,8 @@ def _peaks():
         d = json.loads(p.read_text())
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W board): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "data sheet"}
 
 
 class ClockSampler:
@@ -281,11 +286,16 @@ def measure_model(model_name, args, ctx, sampler, with_roofline=True):
     barrier()
     e0.record()
     for _ in range(args.steps):
-        step(x_dev)
+        last = step(x_dev)
     drain()
     e1.record()
     barrier()
     ms_local = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:
+        # copied now: the graph's output buffer is overwritten by the end-to-end and roofline passes below
+        out_dir = Path(args.dump_outputs)
+        out_dir.mkdir(parents=True, exist_ok=True)
+        np.save(out_dir / f"{model_name}.npy", last.float().cpu().numpy())
     launches = ops.launch_count - launches0
     clocks = sampler.window(mark) if sampler is not None else None
     per_rank_ms = [ms_local / args.steps]
@@ -404,7 +414,7 @@ def run_b200(args):
             "scaling": "weak", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
             "config": {"workload": head["workload"], "global_batch": world * args.batch, "parallelism": f"dp{world}",
                        "cuda_graph": bool(args.graph),
-                       "l2": "per-step working set (154 MB input + >1 GB activations) exceeds the 126 MB L2",
+                       "l2": "per-step working set (154 MB input + >1 GB activations) exceeds the 50 MB L2",
                        "graph_level": head["graph_level"],
                        "collective": ("one NCCL all-gather of the fp32 logits per step, issued asynchronously "
                                       "(double-buffered): ranks are not lock-stepped" if world > 1 else "none"),
@@ -502,6 +512,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the logits of the last timed step of every timed model to DIR/<model>.npy")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--model", default="vit_base_patch16_224")
     ap.add_argument("--batch", type=int, default=256, help="per-GPU batch")
@@ -514,6 +526,8 @@ def main():
     ap.add_argument("--no-graph", dest="graph", action="store_false",
                     help="launch kernels eagerly instead of replaying a captured CUDA graph")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         run_reference(args)
     else:

@@ -1,4 +1,4 @@
-/* tfimm_b200 -- C ABI of the B200 (sm_100a) kernel library behind the tfimm forward path.
+/* tfimm_b200 -- C ABI of the H100 (sm_90a) kernel library behind the tfimm forward path.
  *
  * The reference (martinsbruveris/tensorflow-image-models) has no FFI of its own: its device
  * boundary is inside TensorFlow.  This header is the boundary a maintainer would bind instead
@@ -15,7 +15,7 @@
  *   - every launch takes the cudaStream_t to enqueue on (as void*); calls are asynchronous
  *   - return value: 0 = OK, otherwise a TFIMM_ERR_* code; tfimm_b200_last_error() returns a
  *     thread-local human-readable message.  Nothing here allocates device memory.
- *   - there is NO CPU fallback: without a B200 these calls fail with a CUDA error.
+ *   - there is NO CPU fallback: without an H100 these calls fail with a CUDA error.
  */
 #ifndef TFIMM_B200_H_
 #define TFIMM_B200_H_
@@ -52,13 +52,13 @@ int tfimm_b200_sm_count(void);
 /* Dense / 1x1 conv with fused epilogue:  C = residual + gamma * act(A @ W^T + bias), or with
  * act_after_residual != 0:  C = act(residual + gamma * (A @ W^T + bias))  (ResNet blocks, resnet.py:186-188).
  * A:[M,K] bf16 (ld = lda), W:[N,K] bf16 (ld = ldw), C/residual:[M,N] of out_dtype (bf16|f32);
- * residual may alias C (in-place residual stream).  tcgen05 tensor cores, TMA, fp32 accumulate.
+ * residual may alias C (in-place residual stream).  wgmma tensor cores, TMA, fp32 accumulate.
  * Replaces tf.keras.layers.Dense at tfimm/architectures/vit.py:142-146, swin.py:124-128,343-345,
  * tfimm/layers/transformers.py:192-205, the classifier heads (vit.py:364-368, swin.py:457-461,
  * convnext.py:356-360, efficientnet.py:259-263) and 1x1 Conv2D (efficientnet_blocks.py:412-434,
  * resnet.py:220-248); gamma/residual fuse ConvNeXtBlock's layer-scale + shortcut (convnext.py:226-227).
- * force_block_n: 0 = auto; 64/128/256 = one-CTA kernel with that tile width; 2 = CTA-pair (cta_group::2)
- * 256x256 kernel (testing / A-B measurements). */
+ * force_block_n: 0 = auto; 64/128/256 = that tile width (testing / A-B measurements); 2 = the widest tile,
+ * the same as 256. */
 int tfimm_b200_gemm_bf16(const void* A, int lda, const void* W, int ldw, const float* bias,
                          const float* gamma, const void* residual, int ldr, void* C, int ldc, int M, int N,
                          int K, int act, int act_after_residual, int out_dtype, int force_block_n, void* stream);
@@ -77,8 +77,8 @@ int tfimm_b200_gemm_bf16_gated(const void* A, int lda, const float* gate, int ro
  * A:[M,C] bf16 (the normalised activations), W1:[hidden,C] bf16, W2:[C,hidden] bf16, b1:[hidden], b2:[C], gamma:[C] or
  * NULL (ConvNeXt layer scale), residual / out:[M,C] fp32 (residual may alias out, or be NULL).  C in {96, 128, 192, 256},
  * hidden a multiple of 128: other shapes return TFIMM_B200_UNSUPPORTED and the caller runs two tfimm_b200_gemm_bf16.
- * One CTA pair per 256 rows walks the hidden dimension in chunks of 128: fc1 chunk (tcgen05, cta_group::2) ->
- * bias + activation -> bf16 back into tensor memory -> A operand of the fc2 chunk product; the [M,hidden]
+ * One CTA per 128 rows walks the hidden dimension in chunks of 64: fc1 chunk (wgmma) -> bias + activation -> bf16
+ * register fragments -> A operand of the fc2 chunk product (wgmma with A from registers); the [M,hidden]
  * activations never reach HBM (the hidden tensor is 61 % of the bytes the two-GEMM form moves at C = 128).  The
  * rounding points are those of the two-GEMM form (bf16 hidden, fp32 accumulation in ascending k).
  * Replaces MLP.call (tfimm/layers/transformers.py:208-214) + layer scale + shortcut in ConvNeXtBlock.call
@@ -88,7 +88,7 @@ int tfimm_b200_mlp_bf16(const void* A, int lda, const void* W1, int ldw1, const 
                         int C, int hidden, int act, void* stream);
 
 /* Dense k x k convolution (+ folded-BN bias, activation, optional residual, act(x + shortcut)) as an IMPLICIT GEMM
- * on the tcgen05 tensor cores: tf.keras.layers.ZeroPadding2D(pad) + Conv2D(k, strides) (+ BatchNormalization, act)
+ * on the wgmma tensor cores: tf.keras.layers.ZeroPadding2D(pad) + Conv2D(k, strides) (+ BatchNormalization, act)
  * at tfimm/architectures/resnet.py:129-150 (BasicBlock 3x3), 230-238 (Bottleneck conv2), 486-512 (deep stems).
  * x: NHWC bf16 [B][H][W][C], C % 64 == 0; W: bf16 [N][k*k*C] in (ky, kx, c) order (the TF kernel (kh,kw,cin,cout)
  * flattened and transposed), leading dimension ldw; out / residual: NHWC [B][Ho][Wo][N], bf16 or fp32.
@@ -152,8 +152,8 @@ int tfimm_b200_window_attention_bf16(const void* qkv, void* out, const float* bi
                                      const int* labels, int B, int nw_img, int N, int H, int dh, float scale,
                                      void* stream);
 
-/* Same operator on the tcgen05 tensor cores (head_dim 32, N <= 52 tokens per window): two windows per 128-row UMMA
- * tile, S = Q K^T and O = P V with fp32 accumulators in tensor memory, cp.async row gather / 64-byte row scatter.
+/* Same operator with the bias and mask in the layout the model precomputes for 7 x 7 windows (head_dim 32, N <= 52
+ * tokens per window; the mma.sync kernel above, one warp per (window, head)).
  * bias_pad: fp32 [H][64][64] (the gathered relative-position bias, rows / columns >= N unused);
  * maskbits: uint64 [nw_img][64], bit j of entry (w, i) set when tokens i and j of window w are in different shift
  * regions (the -100 entries of swin.py:249-273), or NULL for unshifted blocks. */
@@ -192,7 +192,7 @@ int tfimm_b200_dwconv_bias_act(const void* x, int dtype, const float* wgt, const
  * efficientnet.py:256, swin.py:456, layers/classifier.py:34). */
 int tfimm_b200_global_avg_pool(const void* x, int dtype, float* out, int B, int HW, int C, void* stream);
 
-/* im2col for dense k x k convolutions (stems, fused-MBConv / ResNet 3x3, 7x7) that then run as tcgen05
+/* im2col for dense k x k convolutions (stems, fused-MBConv / ResNet 3x3, 7x7) that then run as tensor-core
  * GEMMs: out[(b,oy,ox), (ky,kx,c)] = x[b, oy*s+ky-pad_t, ox*s+kx-pad_l, c], zero outside / beyond k*k*C.
  * Replaces the gather half of tf.keras.layers.Conv2D at efficientnet.py:216-222,
  * efficientnet_blocks.py:482-497 (conv_exp), resnet.py:130-137,230-238,506-512.

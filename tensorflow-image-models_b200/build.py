@@ -1,10 +1,10 @@
-"""Builds libtfimm_b200.so (sm_100a only) in-tree with nvcc.
+"""Builds libtfimm_b200.so (sm_90a, H100) in-tree with nvcc.
 
     python tensorflow-image-models_b200/build.py [--force] [--verbose]
 
 The shared object lands next to the ctypes binding
 (``tensorflow-image-models_b200/tfimm/backend/libtfimm_b200.so``) so that it travels to
-the GPU box with the repository snapshot.  nvcc cross-compiles without a GPU.
+wherever the repository tree goes.  nvcc cross-compiles without a GPU.
 """
 import argparse
 import hashlib
@@ -22,7 +22,7 @@ LIB = OUT_DIR / "libtfimm_b200.so"
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC",
@@ -72,7 +72,7 @@ def build(force: bool = False, verbose: bool = False, defines=(), out: Path = No
     if verbose:
         print("\n".join(log))
     link = [NVCC, "-shared", "-o", str(LIB), *[str(o) for _, o, _ in results],
-            "-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+            "-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"]
     res = subprocess.run(link, capture_output=True, text=True)
     if res.returncode != 0:
         sys.stderr.write(res.stdout + res.stderr)
@@ -97,7 +97,7 @@ def _build_variant(defines, out: Path) -> Path:
             sys.stderr.write(res.stderr)
             raise RuntimeError(f"nvcc failed on {obj.stem}")
     res = subprocess.run([NVCC, "-shared", "-o", str(out), *[str(o) for o, _ in results],
-                          "-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"], capture_output=True, text=True)
+                          "-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"], capture_output=True, text=True)
     if res.returncode != 0:
         sys.stderr.write(res.stdout + res.stderr)
         raise RuntimeError("link failed")

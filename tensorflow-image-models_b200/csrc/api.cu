@@ -96,7 +96,7 @@ static inline cudaStream_t S(void* s) { return reinterpret_cast<cudaStream_t>(s)
 
 extern "C" {
 
-const char* tfimm_b200_version(void) { return "tfimm_b200 0.1.0 (sm_100a)"; }
+const char* tfimm_b200_version(void) { return "tfimm_b200 0.1.0 (sm_90a)"; }
 const char* tfimm_b200_last_error(void) { return tfimm::g_last_error; }
 int tfimm_b200_sm_count(void) { return tfimm::sm_count(); }
 

@@ -268,8 +268,6 @@ __global__ void attention_f32_kernel(const float* __restrict__ qkv, float* __res
 
 }  // namespace
 
-int attention_bf16_tc2(const void* qkv, void* out, int B, int N, int H, float scale, cudaStream_t stream);
-
 int attention_bf16(const void* qkv, void* out, int B, int N, int H, int dh, float scale,
                    cudaStream_t stream) {
   TFIMM_CHECK_ARG(B > 0 && N > 0 && H > 0, "attention: bad shape B=%d N=%d H=%d", B, N, H);
@@ -279,9 +277,6 @@ int attention_bf16(const void* qkv, void* out, int B, int N, int H, int dh, floa
   }
   TFIMM_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15u) == 0 && (reinterpret_cast<uintptr_t>(out) & 15u) == 0,
                   "attention: pointers must be 16-byte aligned");
-  // Short sequences (ViT-B/16 @224: N = 197) run on tcgen05 (attention_sm100.cu); longer ones on the resident-KV
-  // mma.sync kernel below.
-  if (N <= 256) return attention_bf16_tc2(qkv, out, B, N, H, scale, stream);
   auto q = reinterpret_cast<const __nv_bfloat16*>(qkv);
   auto o = reinterpret_cast<__nv_bfloat16*>(out);
   // resident K/V + one query tile per CTA must fit 227 KB: 224-row tiles up to N = 784, 128-row tiles up to N = 832

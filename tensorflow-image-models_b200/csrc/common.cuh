@@ -1,4 +1,4 @@
-// Shared device/host helpers for the tfimm_b200 kernel library (sm_100a only).
+// Shared device/host helpers for the tfimm_b200 kernel library (sm_90a).
 //
 // Everything in here is a thin wrapper over a PTX instruction or a small
 // utility used by more than one translation unit.  No torch types, no
@@ -115,7 +115,7 @@ __device__ __forceinline__ float gelu_fast(float x) {
   return x > 0.f ? x - h : -h;
 }
 
-// ---- packed fp32 pairs (Blackwell FFMA2: two fp32 FMAs per issued instruction) ----
+// ---- fp32 pairs: two values carried in one 64-bit register pair, operated on element by element ----
 __device__ __forceinline__ uint64_t pack2(float lo, float hi) {
   uint64_t r;
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -126,32 +126,32 @@ __device__ __forceinline__ void unpack2(uint64_t v, float& lo, float& hi) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float a0, a1, b0, b1, c0, c1;
+  unpack2(a, a0, a1);
+  unpack2(b, b0, b1);
+  unpack2(c, c0, c1);
+  return pack2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ uint64_t mul2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  unpack2(a, a0, a1);
+  unpack2(b, b0, b1);
+  return pack2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t add2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  unpack2(a, a0, a1);
+  unpack2(b, b0, b1);
+  return pack2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 
 // ---- accurate activations for the tensor-core epilogues (packed pairs, groups of FOUR elements) ----
 // The bf16 parity budget (tests/test_parity_budget_gpu.py) needs every value to be right to ~1e-5 BEFORE it is rounded
 // to bf16: a pre-rounding error d flips the rounding of a fraction d/ulp of the elements by a whole ulp, i.e. it adds
-// noise of variance d*ulp against the ulp^2/12 inherent to bf16 storage -- tanh.approx (2^-11) would DOUBLE the noise.
-// (Round 1 shipped one-MUFU tanh.approx forms: 2.5e-4 |x| off for GELU, 12-25 % of the stored values off by an ulp;
-// measured cost of the accurate forms on B200, same box: ViT-B 25.8 -> 25.1 K img/s, ConvNeXt-B 18.3 -> 17.7 K,
-// EfficientNet-B4 9.2 -> 8.6 K.)
+// noise of variance d*ulp against the ulp^2/12 inherent to bf16 storage -- tanh.approx (2^-11) would DOUBLE the noise
+// (one-MUFU tanh.approx forms put 12-25 % of the stored values off by an ulp).
 // Both activations are written as x * sigma with sigma = 1 / (1 + 2^u): one MUFU.EX2 (rel. error 2^-22) and one
-// MUFU.RCP per element.  (A shared reciprocal -- 1 / (d0 d1 d2 d3) and nine multiplications for four quotients, 1.25
-// MUFU per element -- was measured 3 % SLOWER on the fc1 + GELU GEMM: under the board's power cap the currency is
-// instructions executed, not the MUFU pipe; tools/power_probe.py.)
+// MUFU.RCP per element.
 // kSharedRcp: ONE MUFU.RCP for four elements -- 1 / (d0 d1 d2 d3), the four quotients recovered with nine
 // multiplications (u clamped to 28 so that the product stays below 2^127) -- 1.25 MUFU per element instead of 2, for
 // kernels whose activation warps are bound by the MUFU pipe (16 lanes / clk / SM) rather than by issue slots.
@@ -335,7 +335,7 @@ __device__ __forceinline__ void st8(__nv_bfloat16* p, const float (&v)[8]) {
 }
 
 // ----------------------------------------------------------------------------
-// PTX wrappers: shared-memory addresses, mbarrier, TMA, tcgen05.
+// PTX wrappers: shared-memory addresses, mbarrier, TMA, wgmma.
 // ----------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -462,198 +462,33 @@ __device__ __forceinline__ void tma_store_wait_all() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// ---- tcgen05 / TMEM ---------------------------------------------------------
-__device__ __forceinline__ void tcgen05_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols)
-               : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; single-CTA, kind::f16 (bf16/fp16 in, fp32 acc).
-__device__ __forceinline__ void umma_bf16_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                             uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread retire.
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
-}
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// TMEM -> registers: this warp's 32 lanes x 16 consecutive 32-bit columns.
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-// registers -> TMEM: this warp's 32 lanes x 8 consecutive 32-bit columns.
-__device__ __forceinline__ void tmem_st_32x32b_x8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]: A rows live in TMEM lanes, K packed two bf16 per 32-bit column.
-__device__ __forceinline__ void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc,
-                                             uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// Shared-memory matrix descriptor for a K-major bf16 tile whose rows are
-// exactly one 128-byte swizzle span (64 bf16), written by TMA SWIZZLE_128B.
-// Field layout: cute/arch/mma_sm100_desc.hpp (SmemDescriptor).
-//   [0,14)  start address >> 4        [16,30) leading byte offset >> 4 (unused for SW128 K-major)
-//   [32,46) stride byte offset >> 4 (8 rows * 128 B = 1024)   [46,48) version = 1 (sm_100)
-//   [61,64) layout type: 2 = SWIZZLE_128B
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
+// ---- wgmma (warpgroup MMA, sm_90a) -----------------------------------------
+// Shared-memory matrix descriptor for a K-major bf16 tile whose rows are exactly one 128-byte swizzle span (64 bf16),
+// written by TMA SWIZZLE_128B; the tile base must be 1024-byte aligned.
+//   [0,14) start address >> 4   [16,30) leading byte offset >> 4 (unused for swizzled K-major)
+//   [32,46) stride byte offset >> 4 (8 rows * 128 B = 1024)   [62,64) layout: 1 = SWIZZLE_128B
+// Advancing 16 elements along K inside the span is +32 bytes, i.e. +2 on the descriptor.
+__device__ __forceinline__ uint64_t gmma_desc_k_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-
-// Same for an MN-major operand (e.g. V[key][dh] used as B[N = dh][K = key]): rows of 64 bf16 along MN
-// (one 128-byte swizzle span), consecutive K indices 128 bytes apart, 8-row swizzle groups 1024 bytes
-// apart (SBO); LBO = distance between 64-element MN blocks (unused when the MN extent is 64).
-// Canonical layout: cute/atom/mma_traits_sm100.hpp, make_umma_desc<Major::MN>.
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
-// Instruction descriptor for kind::f16 with bf16 A/B (both K-major), fp32 D.
-// Field layout: cute/arch/mma_sm100_desc.hpp (InstrDescriptor).
-__host__ __device__ constexpr uint32_t umma_idesc_bf16_f32(int m, int n, bool b_mn_major = false) {
-  return (1u << 4)                    // c_format = F32
-         | (1u << 7)                  // a_format = BF16
-         | (1u << 10)                 // b_format = BF16
-         | ((b_mn_major ? 1u : 0u) << 16)  // b_major: 0 = K-major, 1 = MN-major
-         | ((uint32_t)(n >> 3) << 17) // n_dim
-         | ((uint32_t)(m >> 4) << 24);  // m_dim
-}
-
-// ---- CTA pair (cta_group::2): two SMs of one TPC execute one 256-row UMMA ------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-// shared::cta address of this CTA -> shared::cluster address of the same offset in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-  return r;
-}
-// Relaxed: callers order their own accesses (tcgen05.fence::before_thread_sync for TMEM reads).  The default
-// .release.cluster form compiles to MEMBAR.ALL.GPU + ERRBAR, which was 15 % of the epilogue warps' time in the
-// CTA-pair GEMM (ncu source view, profiles/r01_ncu_full_gemm_fc1_pair.txt).
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
+// ---- thread-block clusters ----
 __device__ __forceinline__ void cluster_arrive_release() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
 }
 __device__ __forceinline__ void cluster_wait_acquire() {
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// TMA load into THIS CTA's smem whose completion bytes are credited to an mbarrier of either CTA of the pair
-// (bar_cluster = shared::cluster address, normally the leader CTA's "full" barrier).
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst_smem, const void* tmap, uint32_t bar_cluster, int c0,
-                                                 int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst_smem), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar_cluster), "r"(c0), "r"(c1)
-      : "memory");
-}
-// Both CTAs of the pair issue these from the warp with the same index.
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t dst_smem) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-// Leader CTA only.  M = 256: rows 0..127 come from the leader's A tile / go to the leader's TMEM, rows 128..255
-// from / to the peer's; each CTA supplies N/2 rows of B at the same smem offset.
-__device__ __forceinline__ void umma_bf16_ss_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                                  uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on the mbarrier at this smem offset in every CTA of `cta_mask` once the issued MMAs retire.
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(bar), "h"(cta_mask)
-      : "memory");
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 
 // ---- cp.async / ldmatrix / mma.sync (used by the attention kernels) ---------

@@ -24,9 +24,6 @@ int dwconv_bias_act_pairs(const void* x, int dtype, const float* wgt, const floa
 int dwconv_bias_act_tma(const void* x, int dtype, const float* wgt, const float* bias, void* out, float* pool_sum,
                         int B, int H, int W, int C, int ks, int stride, int pad_t, int pad_l, int Ho, int Wo, int act,
                         cudaStream_t stream);
-int dwconv7_ln_tmem(const void* x, int in_dtype, const float* wgt, const float* bias, const float* gamma,
-                    const float* beta, void* out, int out_dtype, int B, int H, int W, int C, float eps,
-                    cudaStream_t stream);
 int dwconv7_ln_cluster(const void* x, int in_dtype, const float* wgt, const float* bias, const float* gamma,
                        const float* beta, void* out, int out_dtype, int B, int H, int W, int C, float eps,
                        cudaStream_t stream);
@@ -263,7 +260,7 @@ __global__ void global_avg_pool_kernel(const T* __restrict__ x, float* __restric
 }
 
 // ----------------------------------------------------------------------------------------------
-// im2col for dense k x k convolutions that are then run as tcgen05 GEMMs
+// im2col for dense k x k convolutions that are then run as tensor-core GEMMs
 // ----------------------------------------------------------------------------------------------
 // out[g][(b, oy, ox)][(ky, kx, c)] = x[b, oy*s + ky - pad_t, ox*s + kx - pad_l, g*cg + c] (0 outside), c < cg = C / G,
 // columns padded with zeros to Kpad.  G = 1 is the plain im2col; column order == TF conv kernel (kh, kw, cin, :)
@@ -648,11 +645,9 @@ int dwconv_ln(const void* x, int in_dtype, const float* wgt, const float* bias, 
   TFIMM_CHECK_ARG(B > 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, "dwconv_ln: need C%%4==0 (C=%d)", C);
   TFIMM_CHECK_ARG(ks == 7, "dwconv_ln: only kernel size 7 is instantiated (got %d)", ks);
   {
-    // Fast paths (fp32 residual stream in, bf16 out): the tensor-memory kernel (dwconv_ln_tmem_sm100.cu) for C a
-    // multiple of 64, else the thread-block-cluster kernel (dwconv_ln_sm100.cu: 32-channel slabs, e.g. C = 96).
-    int st = dwconv7_ln_tmem(x, in_dtype, wgt, bias, gamma, beta, out, out_dtype, B, H, W, C, eps, stream);
-    if (st != kUnsupported) return st;
-    st = dwconv7_ln_cluster(x, in_dtype, wgt, bias, gamma, beta, out, out_dtype, B, H, W, C, eps, stream);
+    // Fast path (fp32 residual stream in, bf16 out): the thread-block-cluster kernel (dwconv_ln_cluster.cu: 64- or
+    // 32-channel slabs per CTA, statistics merged through distributed shared memory).
+    const int st = dwconv7_ln_cluster(x, in_dtype, wgt, bias, gamma, beta, out, out_dtype, B, H, W, C, eps, stream);
     if (st != kUnsupported) return st;
   }
   constexpr int TW = 7;
@@ -701,7 +696,7 @@ int dwconv_bias_act(const void* x, int dtype, const float* wgt, const float* bia
                   "dwconv: kernel size 3/5/7 and stride 1/2 are instantiated (got k=%d s=%d)", ks, stride);
   TFIMM_CHECK_ARG(dtype == kBF16 || dtype == kF32, "dwconv: dtype must be bf16 or f32");
   {
-    // bf16, k in {3,5}: TMA-halo shared-memory kernel (dwconv_act_tma_sm100.cu)
+    // bf16, k in {3,5}: TMA-halo shared-memory kernel (dwconv_act_tma.cu)
     {
       const int st = dwconv_bias_act_tma(x, dtype, wgt, bias, out, pool_sum, B, H, W, C, ks, stride, pad_t, pad_l, Ho,
                                          Wo, act, stream);
@@ -709,7 +704,7 @@ int dwconv_bias_act(const void* x, int dtype, const float* wgt, const float* bia
     }
   }
   {
-    // channel-pair / register-prefetch kernel (dwconv_act_sm100.cu) for k in {3,5}, fp32 and odd shapes; the kernel
+    // channel-pair / register-prefetch kernel (dwconv_act.cu) for k in {3,5}, fp32 and odd shapes; the kernel
     // below is the generic fallback (k = 7).
     const int st = dwconv_bias_act_pairs(x, dtype, wgt, bias, out, pool_sum, B, H, W, C, ks, stride, pad_t, pad_l,
                                          Ho, Wo, act, stream);

@@ -1,9 +1,9 @@
-// Epilogue shared by the tcgen05 GEMM kernels (gemm_sm100.cu: one CTA per tile; gemm2_sm100.cu: CTA pair):
+// Epilogue shared by the wgmma GEMM kernels (gemm_sm90.cu, the fc2 half of mlp_sm90.cu):
 //     C = residual + gamma * act(acc + bias)            (or act(residual + ...) with act_post)
-// One epilogue warp owns 32 accumulator rows (one TMEM lane quarter) and moves them in 128-byte column chunks:
-// tcgen05.ld -> bias/act/gamma on packed fp32 pairs (FFMA2) -> + residual (TMA-prefetched into the warp's own
-// smem slab while the accumulator is loaded and activated) -> 128B-swizzled slab -> TMA store.  The residual may
-// alias the output (in-place fp32 residual stream).
+// applied straight to a warpgroup's accumulator fragments (wgmma.cuh): each thread owns two rows (r, r + 8) and, per
+// 8-column group, two adjacent columns of each, so bias / gamma / activation run on packed fp32 pairs and the residual
+// load and output store are one 4- or 8-byte access per row and group.  The residual may alias the output (in-place
+// fp32 residual stream): every element is read and written by the same thread.
 #pragma once
 #include "common.cuh"
 
@@ -16,52 +16,40 @@ struct GemmParams {
   int act;
   int has_res;
   int act_post;  // 1: activation applied after the residual add (ResNet: act(x + shortcut))
-  // Squeeze-excite gate folded into the A operand (gemm_sm100.cu, gated instances): row m of A is multiplied by
+  void* c;             // output, row stride ldc elements (plain GEMM) or NHWC [B][Ho][Wo][N] (implicit convolution)
+  const void* res;     // residual, same layout as c (row stride ldr), or null
+  long ldc, ldr;
+  // Squeeze-excite gate folded into the A operand (gemm_sm90.cu, gated instances): row m of A is multiplied by
   // a_scale[m / a_rows_per_img][k] (fp32 [a_imgs][K]) and rounded back to bf16 in shared memory, between the TMA load
   // and the MMA -- the values the separate scale_channels pass used to write to HBM.
   const float* a_scale;
   int a_rows_per_img, a_imgs;
-  // Implicit convolution (gemm_sm100.cu): the A operand is not a matrix but the NHWC input itself.  A tile's 128
+  // Implicit convolution (gemm_sm90.cu): the A operand is not a matrix but the NHWC input itself.  A tile's 128
   // rows are a patch of cv_pb images x cv_ph rows x cv_pw columns of OUTPUT pixels; k-block kb is tap
   // (ky, kx) = kb / (C/64) and 64 input channels, fetched as ONE 4-D TMA box whose out-of-bounds elements are
-  // the zero padding.  C and the residual are NHWC too (4-D stores of pw x 32/pw pixel patches per warp).
+  // the zero padding.  C and the residual are NHWC [cv_B][cv_Ho][cv_Wo][N].
   int conv;                  // 0: plain GEMM
   int cv_cblocks;            // C / 64
   int cv_ks, cv_stride, cv_pad;
   int cv_pb, cv_ph, cv_pw;
   int cv_tiles_x, cv_tiles_y;  // patch grid per image group (x fastest, then y, then image group)
+  int cv_B, cv_Ho, cv_Wo;
 };
 
-struct ConvTile {
-  int x, y, b;  // output-pixel coordinates of a warp's first row
-};
-
-constexpr int kEpiSlabBytes = 32 * 128;     // 32 rows x 128 B, one per epilogue warp
-
-// v[j] (+ or *)= vec[n0 + j] on packed pairs; full chunks use 16-byte loads.
-template <int CH, bool kMul>
-__device__ __forceinline__ void apply_vec(uint64_t (&v)[CH / 2], const float* __restrict__ vec, int n0, int N) {
-  if (n0 + CH <= N) {
-#pragma unroll
-    for (int j = 0; j < CH; j += 4) {
-      const float4 b4 = __ldg(reinterpret_cast<const float4*>(vec + n0 + j));
-      if (kMul) {
-        v[j / 2] = mul2(v[j / 2], pack2(b4.x, b4.y));
-        v[j / 2 + 1] = mul2(v[j / 2 + 1], pack2(b4.z, b4.w));
-      } else {
-        v[j / 2] = add2(v[j / 2], pack2(b4.x, b4.y));
-        v[j / 2 + 1] = add2(v[j / 2 + 1], pack2(b4.z, b4.w));
-      }
-    }
-  } else {
-#pragma unroll
-    for (int j = 0; j < CH; j += 2) {
-      const float neutral = kMul ? 1.f : 0.f;
-      const float b0 = (n0 + j < N) ? __ldg(vec + n0 + j) : neutral;
-      const float b1 = (n0 + j + 1 < N) ? __ldg(vec + n0 + j + 1) : neutral;
-      v[j / 2] = kMul ? mul2(v[j / 2], pack2(b0, b1)) : add2(v[j / 2], pack2(b0, b1));
-    }
+// Element offset of output row `r` (0..127) of tile m_blk, or -1 when the row lies outside the output.
+__device__ __forceinline__ long epilogue_row_offset(const GemmParams& p, int m_blk, int r, long ld) {
+  if (p.conv == 0) {
+    const long m = (long)m_blk * 128 + r;
+    return m < p.M ? m * ld : -1;
   }
+  const int tx = m_blk % p.cv_tiles_x, tyb = m_blk / p.cv_tiles_x;
+  const int ty = tyb % p.cv_tiles_y, tb = tyb / p.cv_tiles_y;
+  const int per_img = p.cv_ph * p.cv_pw;
+  const int b = tb * p.cv_pb + r / per_img;
+  const int y = ty * p.cv_ph + (r % per_img) / p.cv_pw;
+  const int x = tx * p.cv_pw + r % p.cv_pw;
+  if (b >= p.cv_B || y >= p.cv_Ho || x >= p.cv_Wo) return -1;
+  return (((long)b * p.cv_Ho + y) * p.cv_Wo + x) * p.N;
 }
 
 template <int NP, bool kSharedRcp = false>
@@ -93,104 +81,80 @@ __device__ __forceinline__ void apply_act_pairs(uint64_t (&v)[NP], int act) {
   }
 }
 
-// One 128-byte column chunk (CH = 128 / sizeof(OutT) columns starting at n0) of this warp's 32 rows (row0..).
-//   t_addr     TMEM address of the chunk's first column in this warp's lane quarter
-//   slab       this warp's 4 KB smem slab (shared::cta address), my_row = generic pointer to this lane's row
-//   res_bar    this warp's residual mbarrier, res_parity = (#chunks this warp has processed) & 1
-//   after_load called once the accumulator values are in registers (caller releases the TMEM stage there)
-//   ct         implicit-convolution mode: where this warp's 32 rows (a pw x 32/pw pixel patch of one image) sit
-//              in the NHWC output; null for a plain row-major C
-//   CHW        columns per chunk: 128 bytes of output per row by default; the CTA-pair kernel's bf16 instance uses
-//              32 columns (64-byte rows, 64B swizzle, 2 KB slabs) so that sixteen epilogue warps fit
-//   kStoresInFlight  1 when the caller passes alternating slabs (two per warp)
-template <typename OutT, int CHW = 128 / (int)sizeof(OutT), int kStoresInFlight = 0, typename AfterLoad>
-__device__ __forceinline__ void epilogue_chunk(const GemmParams& p, uint32_t t_addr, int n0, int row0,
-                                               uint32_t slab, uint8_t* my_row, int lane, uint32_t res_bar,
-                                               uint32_t res_parity, const CUtensorMap* tmap_c,
-                                               const CUtensorMap* tmap_r, const ConvTile* ct,
-                                               AfterLoad after_load) {
-  constexpr int CH = CHW;
-  constexpr int RB = CH * (int)sizeof(OutT);  // bytes per slab row: 128 or 64
-  constexpr int UNITS = RB / 16;
-  static_assert(RB == 128 || RB == 64, "slab rows are 128 or 64 bytes");
-  // TMA swizzle: 16-byte unit j of row r lives at j ^ (r & 7) (SWIZZLE_128B) or j ^ ((r >> 1) & 3) (SWIZZLE_64B)
-  const int sw = RB == 128 ? (lane & 7) : ((lane >> 1) & 3);
-  // the previous store of this warp FROM THIS SLAB must have finished reading it (kStoresInFlight = 1: the caller
-  // alternates between two slabs, so the store issued one chunk ago may still be in flight)
-  if (lane == 0) {
-    tma_store_wait_read<kStoresInFlight>();
+__device__ __forceinline__ uint64_t ld_pair_or(const float* __restrict__ vec, int n, int N, float neutral) {
+  if (n + 1 < N) {
+    const float2 f = __ldg(reinterpret_cast<const float2*>(vec + n));
+    return pack2(f.x, f.y);
+  }
+  return pack2(n < N ? __ldg(vec + n) : neutral, neutral);
+}
+
+__device__ __forceinline__ uint64_t ld_out_pair(const float* p, bool two) {
+  if (two) {
+    const float2 f = *reinterpret_cast<const float2*>(p);
+    return pack2(f.x, f.y);
+  }
+  return pack2(*p, 0.f);
+}
+__device__ __forceinline__ uint64_t ld_out_pair(const __nv_bfloat16* p, bool two) {
+  if (two) {
+    const float2 f = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p));
+    return pack2(f.x, f.y);
+  }
+  return pack2(__bfloat162float(*p), 0.f);
+}
+__device__ __forceinline__ void st_out_pair(float* p, uint64_t v, bool two) {
+  float a, b;
+  unpack2(v, a, b);
+  if (two) *reinterpret_cast<float2*>(p) = make_float2(a, b);
+  else *p = a;
+}
+__device__ __forceinline__ void st_out_pair(__nv_bfloat16* p, uint64_t v, bool two) {
+  float a, b;
+  unpack2(v, a, b);
+  if (two) *reinterpret_cast<uint32_t*>(p) = pack_bf16x2(a, b);
+  else *p = __float2bfloat16_rn(a);
+}
+
+// Epilogue of one warpgroup's 64 x BN accumulator (BN / 2 fp32 per thread, wgmma.cuh layout) of tile (m_blk, n_blk);
+// the warpgroup's rows start at tile row `wg_row0`.  Columns are handled 8 at a time (four values per thread: rows r and
+// r + 8, columns c and c + 1), which is the granularity of the four-element activations.
+template <typename OutT, int BN>
+__device__ __forceinline__ void epilogue_frag(const GemmParams& p, float (&acc)[BN / 2], int m_blk, int n_blk,
+                                              int wg_row0) {
+  const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
+  const int r = wg_row0 + wq * 16 + (lane >> 2);
+  const long off_c[2] = {epilogue_row_offset(p, m_blk, r, p.ldc), epilogue_row_offset(p, m_blk, r + 8, p.ldc)};
+  const long off_r[2] = {p.has_res ? epilogue_row_offset(p, m_blk, r, p.ldr) : -1,
+                         p.has_res ? epilogue_row_offset(p, m_blk, r + 8, p.ldr) : -1};
+  OutT* __restrict__ C = reinterpret_cast<OutT*>(p.c);
+  const OutT* R = reinterpret_cast<const OutT*>(p.res);
+#pragma unroll
+  for (int g = 0; g < BN / 8; ++g) {
+    const int n = n_blk * BN + g * 8 + 2 * (lane & 3);
+    if (n_blk * BN + g * 8 >= p.N) break;
+    const bool in = n < p.N, two = n + 1 < p.N;
+    uint64_t v[2] = {pack2(acc[4 * g + 0], acc[4 * g + 1]), pack2(acc[4 * g + 2], acc[4 * g + 3])};
+    if (p.bias != nullptr) {
+      const uint64_t b = ld_pair_or(p.bias, n, p.N, 0.f);
+      v[0] = add2(v[0], b);
+      v[1] = add2(v[1], b);
+    }
+    if (!p.act_post) apply_act_pairs(v, p.act);
+    if (p.gamma != nullptr) {
+      const uint64_t s = ld_pair_or(p.gamma, n, p.N, 1.f);
+      v[0] = mul2(v[0], s);
+      v[1] = mul2(v[1], s);
+    }
     if (p.has_res) {
-      mbar_expect_tx(res_bar, 32 * RB);
-      if (ct == nullptr) tma_load_2d(slab, tmap_r, res_bar, n0, row0);
-      else tma_load_4d(slab, tmap_r, res_bar, n0, ct->x, ct->y, ct->b);
-    }
-  }
-  __syncwarp();
-  uint64_t v[CH / 2];
-  {
-    uint32_t r[32];
 #pragma unroll
-    for (int h = 0; h < CH / 32; ++h) {
-      tmem_ld_32x32b_x32(t_addr + (uint32_t)(h * 32), r);
-      tmem_ld_wait();
-#pragma unroll
-      for (int j = 0; j < 16; ++j)
-        v[h * 16 + j] = pack2(__uint_as_float(r[2 * j]), __uint_as_float(r[2 * j + 1]));
+      for (int h = 0; h < 2; ++h)
+        if (in && off_r[h] >= 0) v[h] = add2(v[h], ld_out_pair(R + off_r[h] + n, two));
     }
-  }
-  after_load();
-  if (p.bias != nullptr) apply_vec<CH, false>(v, p.bias, n0, p.N);
-  if (!p.act_post) apply_act_pairs(v, p.act);
-  if (p.gamma != nullptr) apply_vec<CH, true>(v, p.gamma, n0, p.N);
-  if (p.has_res) {
-    mbar_wait(res_bar, res_parity);
+    if (p.act_post) apply_act_pairs(v, p.act);
 #pragma unroll
-    for (int j = 0; j < UNITS; ++j) {
-      const uint4 u = *reinterpret_cast<const uint4*>(my_row + ((j ^ sw) << 4));
-      if constexpr (sizeof(OutT) == 2) {
-        const float2 f0 = unpack_bf16x2(u.x), f1 = unpack_bf16x2(u.y);
-        const float2 f2 = unpack_bf16x2(u.z), f3 = unpack_bf16x2(u.w);
-        v[4 * j + 0] = add2(v[4 * j + 0], pack2(f0.x, f0.y));
-        v[4 * j + 1] = add2(v[4 * j + 1], pack2(f1.x, f1.y));
-        v[4 * j + 2] = add2(v[4 * j + 2], pack2(f2.x, f2.y));
-        v[4 * j + 3] = add2(v[4 * j + 3], pack2(f3.x, f3.y));
-      } else {
-        v[2 * j + 0] = add2(v[2 * j + 0], pack2(__uint_as_float(u.x), __uint_as_float(u.y)));
-        v[2 * j + 1] = add2(v[2 * j + 1], pack2(__uint_as_float(u.z), __uint_as_float(u.w)));
-      }
-    }
-  }
-  if (p.act_post) apply_act_pairs(v, p.act);
-#pragma unroll
-  for (int j = 0; j < UNITS; ++j) {
-    uint4 u;
-    if constexpr (sizeof(OutT) == 2) {
-      float a0, a1, a2, a3, a4, a5, a6, a7;
-      unpack2(v[4 * j + 0], a0, a1);
-      unpack2(v[4 * j + 1], a2, a3);
-      unpack2(v[4 * j + 2], a4, a5);
-      unpack2(v[4 * j + 3], a6, a7);
-      u.x = pack_bf16x2(a0, a1);
-      u.y = pack_bf16x2(a2, a3);
-      u.z = pack_bf16x2(a4, a5);
-      u.w = pack_bf16x2(a6, a7);
-    } else {
-      float a0, a1, a2, a3;
-      unpack2(v[2 * j + 0], a0, a1);
-      unpack2(v[2 * j + 1], a2, a3);
-      u.x = __float_as_uint(a0);
-      u.y = __float_as_uint(a1);
-      u.z = __float_as_uint(a2);
-      u.w = __float_as_uint(a3);
-    }
-    *reinterpret_cast<uint4*>(my_row + ((j ^ sw) << 4)) = u;
-  }
-  fence_proxy_async_smem();
-  __syncwarp();
-  if (lane == 0) {
-    if (ct == nullptr) tma_store_2d(tmap_c, slab, n0, row0);
-    else tma_store_4d(tmap_c, slab, n0, ct->x, ct->y, ct->b);
-    tma_store_commit();
+    for (int h = 0; h < 2; ++h)
+      if (in && off_c[h] >= 0) st_out_pair(C + off_c[h] + n, v[h], two);
   }
 }
 

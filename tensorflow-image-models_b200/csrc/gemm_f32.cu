@@ -1,7 +1,7 @@
-// fp32 SIMT GEMM with the same fused epilogue as the tcgen05 kernel:
+// fp32 SIMT GEMM with the same fused epilogue as the tensor-core kernel:
 //     C = residual + gamma * act(A @ W^T + bias)       A:[M,K]  W:[N,K]  (fp32, K contiguous)
 // Used only by precision="fp32" (the 1e-5 structural-parity mode of the engine);
-// the performance path is gemm_sm100.cu.  64x64 tiles, 4x4 micro-tiles, BK = 16.
+// the performance path is gemm_sm90.cu.  64x64 tiles, 4x4 micro-tiles, BK = 16.
 #include "common.cuh"
 
 namespace tfimm {

@@ -5,10 +5,8 @@
 // Call sites: the 1x1 convolutions of EfficientNet's first stages and stems -- (K, N) = (27->32, 48), (48, 24),
 // (24, 144), (32, 192), (56, 336) with M up to 9.2 M pixels at 380 px -- and the patch-embedding GEMMs (K = 48) of
 // Swin / ConvNeXt (tfimm/architectures/efficientnet_blocks.py:412-434, layers/transformers.py:131-139).  At K <= 64
-// the work is ~40 flop per byte: HBM-bound, with the activation (one MUFU.EX2 per element) as the second term.  The
-// persistent tcgen05 kernel handles such shapes one 128 x 64 tile per barrier round trip (TMA -> UMMA -> tcgen05.ld
-// -> TMA store, ~2.5 us per tile): B4's 9.2 M x 24 -> 144 expansion ran at 1.5 TB/s (2.06 ms of a 28 ms forward).
-// Here the whole weight matrix sits in shared memory for the life of the CTA, warps stream 16-row slices of A through
+// the work is ~40 flop per byte: HBM-bound, with the activation (one MUFU.EX2 per element) as the second term.  A tile
+// pipeline (TMA -> tensor core -> epilogue) pays a barrier round trip per 128 x 64 tile on such shapes.  Here the whole weight matrix sits in shared memory for the life of the CTA, warps stream 16-row slices of A through
 // cp.async double buffers, multiply on mma.sync (HMMA -- the tensor pipe is idle either way at this intensity) and
 // store their fragments directly; occupancy (up to 24 warps / SM), not a pipeline, hides the latency.
 #include "common.cuh"
@@ -165,7 +163,7 @@ gemm_bf16_skinny_kernel(const __nv_bfloat16* __restrict__ A, int lda, const __nv
 
 }  // namespace
 
-// Returns kUnsupported (without setting an error) for shapes outside this kernel: the caller uses the tcgen05 path.
+// Returns kUnsupported (without setting an error) for shapes outside this kernel: the caller uses the wgmma path.
 int gemm_bf16_skinny(const void* A, int lda, const void* W, int ldw, const float* bias, const void* residual, int ldr,
                      void* C, int ldc, int M, int N, int K, int act, cudaStream_t stream, const float* gate,
                      int rows_per_img, int imgs) {

@@ -1,0 +1,389 @@
+// Dense contraction for the tfimm forward path on sm_90a:
+//
+//     C[M,N] = residual[M,N] + gamma[N] * act(A[M,K] @ W[N,K]^T + bias[N])
+//
+// This single kernel replaces every tf.keras.layers.Dense and 1x1 Conv2D the
+// reference calls on the hot path (qkv/proj: tfimm/architectures/vit.py:142-146,
+// swin.py:124-128; fc1/fc2: tfimm/layers/transformers.py:192-205; heads:
+// vit.py:364-368, convnext.py:356-360; 1x1 convs: efficientnet_blocks.py:412-434,
+// resnet.py:220-248) plus the patchify convolutions once their input has been
+// gathered (layers/transformers.py:131-139, convnext.py:259-266,319-326).
+//
+// Design (one 128 x BLOCK_N output tile per CTA, warp-specialised):
+//   warps 0..7  two consumer warpgroups, 64 tile rows each: wgmma m64 x BLOCK_N x k16 from the swizzled smem ring,
+//               fp32 accumulators in registers, one wgmma group kept in flight (the stage of the group before it is
+//               released as soon as it retires); then the epilogue straight from the fragments (gemm_epilogue.cuh)
+//   warp 8      TMA producer: A/W tiles -> 128B-swizzled smem ring (mbarrier full/empty)
+//   warps 9..12 (gated instances only) squeeze-excite gate applied to the A tile in smem before the MMA reads it
+#include "gemm_epilogue.cuh"
+#include "wgmma.cuh"
+
+namespace tfimm {
+
+namespace {
+
+constexpr int kBlockM = 128;
+constexpr int kBlockK = 64;   // 64 bf16 = one 128-byte swizzle span
+constexpr int kConsumerThreads = 256;
+constexpr int kProducerWarp = kConsumerThreads / 32;
+constexpr int kNumGateWarps = 4;   // gated instances only: one thread per A-tile row
+
+template <int BLOCK_N>
+struct GemmCfg {
+  static constexpr int kABytes = kBlockM * kBlockK * 2;
+  static constexpr int kBBytes = BLOCK_N * kBlockK * 2;
+  static constexpr int kStageBytes = kABytes + kBBytes;
+  static constexpr int kStages = 4;   // 192 / 128 / 96 KB: BLOCK_N = 64 leaves room for two CTAs per SM
+  static constexpr int kNumBarriers = 3 * kStages;   // full, empty, ready (gated)
+  static constexpr int kSmemBytes = kStages * kStageBytes + kNumBarriers * 8 + 1024 /*alignment slack*/;
+};
+
+template <int BLOCK_N, bool kGated>
+constexpr int gemm_threads() { return kConsumerThreads + 32 + (kGated ? 32 * kNumGateWarps : 0); }
+
+template <int BLOCK_N, typename OutT, bool kGated = false>
+__global__ void __launch_bounds__(gemm_threads<BLOCK_N, kGated>(), (BLOCK_N == 64 && !kGated) ? 2 : 1)
+gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                       const GemmParams p) {
+  using Cfg = GemmCfg<BLOCK_N>;
+  constexpr int kStages = Cfg::kStages;
+
+  extern __shared__ uint8_t smem_raw[];
+  // SWIZZLE_128B tiles need 1024-byte alignment.
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t smem_tiles = smem_base;
+  const uint32_t smem_bars = smem_base + kStages * Cfg::kStageBytes;
+  auto full_bar = [&](int s) { return smem_bars + 8u * s; };
+  auto empty_bar = [&](int s) { return smem_bars + 8u * (kStages + s); };
+  auto ready_bar = [&](int s) { return smem_bars + 8u * (2 * kStages + s); };
+
+  const int warp_idx = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+
+  if (warp_idx == kProducerWarp && lane == 0) {
+    prefetch_tmap(&tmap_a);
+    prefetch_tmap(&tmap_b);
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(full_bar(s), 1);
+      mbar_init(empty_bar(s), 2);   // one arrival per consumer warpgroup
+      mbar_init(ready_bar(s), 1);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  const int num_n_tiles = (p.N + BLOCK_N - 1) / BLOCK_N;
+  const int m_blk = blockIdx.x / num_n_tiles, n_blk = blockIdx.x % num_n_tiles;
+  const int num_k_blocks = (p.K + kBlockK - 1) / kBlockK;
+
+  if (warp_idx == kProducerWarp) {
+    // ------------------------------ TMA producer ------------------------------
+    if (lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int kb = 0; kb < num_k_blocks; ++kb) {
+        mbar_wait(empty_bar(stage), phase ^ 1u);
+        const uint32_t sa = smem_tiles + stage * Cfg::kStageBytes;
+        const uint32_t sb = sa + Cfg::kABytes;
+        mbar_expect_tx(full_bar(stage), Cfg::kStageBytes);
+        if (p.conv == 0) {
+          tma_load_2d(sa, &tmap_a, full_bar(stage), kb * kBlockK, m_blk * kBlockM);
+        } else {
+          // implicit convolution: tap (ky, kx) and a 64-channel slice of the input patch; padding = OOB zero fill
+          const int tap = kb / p.cv_cblocks, cb = kb - tap * p.cv_cblocks;
+          const int ky = tap / p.cv_ks, kx = tap - ky * p.cv_ks;
+          const int tx = m_blk % p.cv_tiles_x, tyb = m_blk / p.cv_tiles_x;
+          const int ty = tyb % p.cv_tiles_y, tb = tyb / p.cv_tiles_y;
+          tma_load_4d(sa, &tmap_a, full_bar(stage), cb * kBlockK, tx * p.cv_pw * p.cv_stride + kx - p.cv_pad,
+                      ty * p.cv_ph * p.cv_stride + ky - p.cv_pad, tb * p.cv_pb);
+        }
+        tma_load_2d(sb, &tmap_b, full_bar(stage), kb * kBlockK, n_blk * BLOCK_N);
+        if (++stage == kStages) { stage = 0; phase ^= 1u; }
+      }
+    }
+  } else if (kGated && warp_idx > kProducerWarp) {
+    // ------------------------- A-operand gate (squeeze-excite) -------------------------
+    // Each of the four warps owns every fourth k-block (a whole 128 x 64 tile), so four stages are being rescaled at
+    // any time.  lane = one 16-byte chunk column (8 contraction indices) x 32 rows 4 apart: the gate values of a lane
+    // change only when its rows cross into the next image; a quarter-warp touches one whole 128-byte row (no bank
+    // conflicts under the 128B swizzle).  x * gate in fp32, back as bf16 -- the rounding of the separate scale pass
+    // (csrc/conv.cu, scale_channels_kernel) -- then the proxy fence that makes the generic-proxy writes visible to the
+    // tensor core's async-proxy reads, and one arrive on the stage's "ready" barrier.
+    const int wt = warp_idx - kProducerWarp - 1;
+    const int c = lane & 7, r0 = lane >> 3;
+    auto load_gate = [&](int img, int k0, float4& ga, float4& gb) {
+      const float* g = p.a_scale + (long)img * p.K + k0;
+      ga = __ldg(reinterpret_cast<const float4*>(g));
+      gb = __ldg(reinterpret_cast<const float4*>(g + 4));
+    };
+    const long row_first = (long)m_blk * kBlockM + r0;
+    long im0 = row_first / p.a_rows_per_img;
+    im0 = im0 < p.a_imgs ? im0 : p.a_imgs - 1;            // rows past M are zero-filled: any gate row will do
+    const int img0 = (int)im0;
+    const long bound0 = (im0 + 1) * p.a_rows_per_img - (long)m_blk * kBlockM;   // first tile row of the next image
+    int stage = 0, turn = 0;   // stage / owner of the NEXT k-block
+    uint32_t phase = 0;
+    for (int kb = 0; kb < num_k_blocks; ++kb) {
+      if (turn == wt) {
+        const int k0 = kb * kBlockK + c * 8;
+        const bool valid = k0 < p.K;                       // K % 8 == 0: a chunk is inside or outside as a whole
+        float4 ga = make_float4(0.f, 0.f, 0.f, 0.f), gb = ga;
+        if (valid) load_gate(img0, k0, ga, gb);
+        mbar_wait(full_bar(stage), phase);
+        if (valid) {
+          const uint32_t sa = smem_tiles + stage * Cfg::kStageBytes;
+          int cur = img0;
+          long bound = bound0;
+#pragma unroll 1
+          for (int b8 = 0; b8 < 4; ++b8) {
+            uint4 u[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              const int r = r0 + 4 * (8 * b8 + i);
+              asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];"
+                           : "=r"(u[i].x), "=r"(u[i].y), "=r"(u[i].z), "=r"(u[i].w)
+                           : "r"(sa + (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4))));
+            }
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              const int r = r0 + 4 * (8 * b8 + i);
+              if (r >= bound && cur < p.a_imgs - 1) {
+                do { ++cur; bound += p.a_rows_per_img; } while (r >= bound && cur < p.a_imgs - 1);
+                load_gate(cur, k0, ga, gb);
+              }
+              const float2 x0 = unpack_bf16x2(u[i].x), x1 = unpack_bf16x2(u[i].y), x2 = unpack_bf16x2(u[i].z),
+                           x3 = unpack_bf16x2(u[i].w);
+              const uint32_t o0 = pack_bf16x2(x0.x * ga.x, x0.y * ga.y), o1 = pack_bf16x2(x1.x * ga.z, x1.y * ga.w);
+              const uint32_t o2 = pack_bf16x2(x2.x * gb.x, x2.y * gb.y), o3 = pack_bf16x2(x3.x * gb.z, x3.y * gb.w);
+              asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(sa + (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4))),
+                           "r"(o0), "r"(o1), "r"(o2), "r"(o3)
+                           : "memory");
+            }
+          }
+        }
+        fence_proxy_async_smem();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(ready_bar(stage));
+      }
+      turn = turn + 1 == kNumGateWarps ? 0 : turn + 1;
+      if (++stage == kStages) { stage = 0; phase ^= 1u; }
+    }
+  } else if (warp_idx < kProducerWarp) {
+    // ------------------------------- consumers -------------------------------
+    const int wg = warp_idx >> 2;   // warpgroup: tile rows 64 wg .. 64 wg + 63
+    const bool releaser = (threadIdx.x & 127) == 0;
+    float acc[BLOCK_N / 2];
+#pragma unroll
+    for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
+    int stage = 0, prev = 0;
+    uint32_t phase = 0;
+    for (int kb = 0; kb < num_k_blocks; ++kb) {
+      mbar_wait(kGated ? ready_bar(stage) : full_bar(stage), phase);   // gated: the A tile has been rescaled
+      const uint32_t sa = smem_tiles + stage * Cfg::kStageBytes;
+      const uint64_t da = gmma_desc_k_sw128(sa + (uint32_t)wg * (64 * 128));
+      const uint64_t db = gmma_desc_k_sw128(sa + Cfg::kABytes);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kBlockK / 16; ++k)
+        wgmma_ss<BLOCK_N>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (uint32_t)((kb | k) != 0));
+      wgmma_commit();
+      // the group issued one k-block ago has retired: its stage may be refilled
+      wgmma_wait<1>();
+      if (kb > 0 && releaser) mbar_arrive(empty_bar(prev));
+      prev = stage;
+      if (++stage == kStages) { stage = 0; phase ^= 1u; }
+    }
+    wgmma_wait<0>();
+    if (releaser) mbar_arrive(empty_bar(prev));
+    epilogue_frag<OutT, BLOCK_N>(p, acc, m_blk, n_blk, wg * 64);
+  }
+}
+
+// ------------------------------ host side -----------------------------------
+// Output / residual: 16-byte aligned base and row stride (vector epilogue accesses, as the layout of every caller).
+int check_out(const void* C, long ldc, const void* residual, long ldr, int esize) {
+  TFIMM_CHECK_ARG((reinterpret_cast<uintptr_t>(C) & 15u) == 0 && (ldc * esize) % 16 == 0,
+                  "gemm: C must be 16-byte aligned with a row stride of a multiple of 16 bytes");
+  TFIMM_CHECK_ARG(residual == nullptr || ((reinterpret_cast<uintptr_t>(residual) & 15u) == 0 && (ldr * esize) % 16 == 0),
+                  "gemm: residual must be 16-byte aligned with a row stride of a multiple of 16 bytes");
+  return kOk;
+}
+
+template <int BLOCK_N, typename OutT, bool kGated = false>
+int launch_gemm(const void* A, int lda, const void* W, int ldw, const void* residual, int ldr, void* C, int ldc,
+                GemmParams p, cudaStream_t stream) {
+  const int M = p.M, N = p.N, K = p.K;
+  using Cfg = GemmCfg<BLOCK_N>;
+  CUtensorMap ta, tb;
+  int st;
+  if ((st = check_out(C, ldc, residual, ldr, (int)sizeof(OutT))) != kOk) return st;
+  if ((st = make_tmap_2d(&ta, A, kBF16, M, K, lda, kBlockM, kBlockK, "A")) != kOk) return st;
+  if ((st = make_tmap_2d(&tb, W, kBF16, N, K, ldw, BLOCK_N, kBlockK, "W")) != kOk) return st;
+  p.c = C; p.res = residual; p.ldc = ldc; p.ldr = ldr;
+  auto kernel = gemm_bf16_wgmma_kernel<BLOCK_N, OutT, kGated>;
+  static unsigned long long attr_devs = 0;  // per instantiation
+  if (first_use_on_device(attr_devs)) {
+    TFIMM_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+  }
+  const long tiles = (long)((M + kBlockM - 1) / kBlockM) * ((N + BLOCK_N - 1) / BLOCK_N);
+  kernel<<<(unsigned)tiles, gemm_threads<BLOCK_N, kGated>(), Cfg::kSmemBytes, stream>>>(ta, tb, p);
+  TFIMM_LAUNCH_OK("gemm_bf16_wgmma_kernel");
+  return kOk;
+}
+
+int pick_block_n(int M, int N);
+
+// Implicit k x k convolution on the tensor cores: same kernel, A tensor map = the NHWC input (rank 4, traversal
+// stride = conv stride), C / residual = the NHWC output.  See GemmParams::conv.
+template <int BLOCK_N, typename OutT>
+int launch_conv(const void* x, const void* W, int ldw, const void* residual, void* out, int B, int H, int Wd, int C,
+                int Ho, int Wo, GemmParams p, cudaStream_t stream) {
+  using Cfg = GemmCfg<BLOCK_N>;
+  const int N = p.N, s = p.cv_stride;
+  CUtensorMap ta, tb;
+  int st;
+  if ((st = check_out(out, N, residual, N, (int)sizeof(OutT))) != kOk) return st;
+  {
+    const uint64_t dims[4] = {(uint64_t)C, (uint64_t)Wd, (uint64_t)H, (uint64_t)B};
+    const uint64_t strides[3] = {(uint64_t)C * 2, (uint64_t)Wd * C * 2, (uint64_t)H * Wd * C * 2};
+    const uint32_t box[4] = {(uint32_t)kBlockK, (uint32_t)(p.cv_pw * s), (uint32_t)(p.cv_ph * s), (uint32_t)p.cv_pb};
+    const uint32_t estr[4] = {1u, (uint32_t)s, (uint32_t)s, 1u};
+    if ((st = make_tmap(&ta, x, kBF16, 4, dims, strides, box, "conv input", 128, estr)) != kOk) return st;
+  }
+  if ((st = make_tmap_2d(&tb, W, kBF16, N, p.K, ldw, BLOCK_N, kBlockK, "conv weights")) != kOk) return st;
+  p.c = out; p.res = residual; p.ldc = N; p.ldr = N;
+  p.cv_B = B; p.cv_Ho = Ho; p.cv_Wo = Wo;
+  auto kernel = gemm_bf16_wgmma_kernel<BLOCK_N, OutT>;
+  static unsigned long long attr_devs = 0;  // per instantiation
+  if (first_use_on_device(attr_devs)) {
+    TFIMM_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+  }
+  const long tiles = (long)(p.M / kBlockM) * ((N + BLOCK_N - 1) / BLOCK_N);
+  kernel<<<(unsigned)tiles, gemm_threads<BLOCK_N, false>(), Cfg::kSmemBytes, stream>>>(ta, tb, p);
+  TFIMM_LAUNCH_OK("gemm_bf16_wgmma_kernel (implicit convolution)");
+  return kOk;
+}
+
+int pick_block_n(int M, int N) {
+  const int sms = sm_count() > 0 ? sm_count() : 132;  // no device (host-side shape queries): H100 SXM
+  const int mt = (M + kBlockM - 1) / kBlockM;
+  int best = 256;
+  double best_cost = 1e30;
+  for (int bn : {256, 128, 64}) {
+    const int nt = (N + bn - 1) / bn;
+    const long tiles = (long)mt * nt;
+    // BLOCK_N = 64 runs two CTAs per SM
+    const int slots = bn == 64 ? 2 * sms : sms;
+    const long waves = (tiles + slots - 1) / slots;
+    // time ~ waves * per-tile MMA time (prop. to bn, halved per CTA when two share an SM); small preference for wide
+    // tiles, which load less operand data per MMA
+    const double cost = (double)waves * (bn == 64 ? 2 * bn : bn) * (bn == 256 ? 1.0 : (bn == 128 ? 1.04 : 1.10));
+    if (cost < best_cost) { best_cost = cost; best = bn; }
+  }
+  return best;
+}
+
+}  // namespace
+
+int gemm_bf16_skinny(const void* A, int lda, const void* W, int ldw, const float* bias, const void* residual, int ldr,
+                     void* C, int ldc, int M, int N, int K, int act, cudaStream_t stream, const float* gate = nullptr,
+                     int rows_per_img = 1, int imgs = 1);
+
+int gemm_bf16_dispatch(const void* A, int lda, const void* W, int ldw, const float* bias,
+                       const float* gamma, const void* residual, int ldr, void* C, int ldc, int M,
+                       int N, int K, int act, int act_post, int out_dtype, int force_block_n, cudaStream_t stream) {
+  TFIMM_CHECK_ARG(M > 0 && N > 0 && K > 0, "gemm: M, N, K must be positive (got %d %d %d)", M, N, K);
+  TFIMM_CHECK_ARG(out_dtype == kBF16 || out_dtype == kF32, "gemm: out_dtype must be bf16 or f32");
+  TFIMM_CHECK_ARG(K % 8 == 0, "gemm: K must be a multiple of 8 (got %d)", K);
+  TFIMM_CHECK_ARG(bias == nullptr || (reinterpret_cast<uintptr_t>(bias) & 15u) == 0, "gemm: bias must be 16-byte aligned");
+  TFIMM_CHECK_ARG(gamma == nullptr || (reinterpret_cast<uintptr_t>(gamma) & 15u) == 0, "gemm: gamma must be 16-byte aligned");
+  if (force_block_n == 0 && K <= 64 && out_dtype == kBF16 && gamma == nullptr && act_post == 0) {
+    // short contraction: streaming mma.sync kernel (gemm_skinny.cu); kUnsupported = shape outside its envelope
+    const int st = gemm_bf16_skinny(A, lda, W, ldw, bias, residual, ldr, C, ldc, M, N, K, act, stream);
+    if (st != kUnsupported) return st;
+  }
+  GemmParams p{};
+  p.M = M; p.N = N; p.K = K;
+  p.bias = bias; p.gamma = gamma; p.act = act; p.has_res = residual != nullptr ? 1 : 0; p.act_post = act_post;
+  // force_block_n: 0 = choose; 64/128/256 = that tile width; 2 = the widest tile (256)
+  const int bn = force_block_n == 2 ? 256 : (force_block_n > 0 ? force_block_n : pick_block_n(M, N));
+#define TFIMM_GEMM_CASE(BN)                                                                         \
+  case BN:                                                                                          \
+    return out_dtype == kBF16 ? launch_gemm<BN, __nv_bfloat16>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream) \
+                              : launch_gemm<BN, float>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream);
+  switch (bn) {
+    TFIMM_GEMM_CASE(256)
+    TFIMM_GEMM_CASE(128)
+    TFIMM_GEMM_CASE(64)
+    default:
+      set_last_error("gemm: unsupported block_n %d", bn);
+      return kInvalidArgument;
+  }
+#undef TFIMM_GEMM_CASE
+}
+
+// Dense layer whose input rows are first multiplied by a per-image channel gate (squeeze-excite): the projection
+// convolutions after SEModule (tfimm/layers/attention.py, efficientnet_blocks.py:241-248, 438-453).  bf16 out.
+int gemm_bf16_gated_dispatch(const void* A, int lda, const float* gate, int rows_per_img, int imgs, const void* W, int ldw,
+                             const float* bias, const void* residual, int ldr, void* C, int ldc, int M, int N, int K,
+                             int act, cudaStream_t stream) {
+  TFIMM_CHECK_ARG(M > 0 && N > 0 && K > 0 && K % 8 == 0, "gemm_gated: need K %% 8 == 0 (got M=%d N=%d K=%d)", M, N, K);
+  TFIMM_CHECK_ARG(gate != nullptr && rows_per_img > 0 && imgs > 0 && (reinterpret_cast<uintptr_t>(gate) & 15u) == 0,
+                  "gemm_gated: gate [imgs][K] fp32, 16-byte aligned");
+  TFIMM_CHECK_ARG(bias == nullptr || (reinterpret_cast<uintptr_t>(bias) & 15u) == 0, "gemm_gated: bias must be 16-byte aligned");
+  if (K <= 64) {   // short contraction: the streaming kernel scales its A fragments in registers
+    const int st = gemm_bf16_skinny(A, lda, W, ldw, bias, residual, ldr, C, ldc, M, N, K, act, stream, gate, rows_per_img,
+                                    imgs);
+    if (st != kUnsupported) return st;
+  }
+  GemmParams p{};
+  p.M = M; p.N = N; p.K = K;
+  p.bias = bias; p.act = act; p.has_res = residual != nullptr ? 1 : 0;
+  p.a_scale = gate; p.a_rows_per_img = rows_per_img; p.a_imgs = imgs;
+  // at most 128 columns: the gate warps leave the consumers too few registers for a 256-wide accumulator
+  switch (pick_block_n(M, N)) {
+    case 256:
+    case 128: return launch_gemm<128, __nv_bfloat16, true>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream);
+    default: return launch_gemm<64, __nv_bfloat16, true>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream);
+  }
+}
+
+// k x k convolution (stride 1 or 2, symmetric padding (k-1)/2... given as `pad`) + bias + activation (+ residual),
+// NHWC bf16 in, NHWC bf16/fp32 out, W[N][k*k*C] in (ky, kx, c) order: implicit GEMM, no im2col matrix in HBM.
+int conv_bf16_dispatch(const void* x, const void* W, int ldw, const float* bias, const void* residual, void* out,
+                       int B, int H, int Wd, int C, int N, int ks, int stride, int pad, int act, int act_post,
+                       int out_dtype, cudaStream_t stream) {
+  TFIMM_CHECK_ARG(B > 0 && H > 0 && Wd > 0 && C > 0 && C % 64 == 0, "conv: C must be a multiple of 64 (got %d)", C);
+  TFIMM_CHECK_ARG(ks >= 1 && ks <= 7 && (stride == 1 || stride == 2) && pad >= 0 && pad < ks, "conv: bad geometry");
+  TFIMM_CHECK_ARG(N > 0 && N % 8 == 0, "conv: N must be a multiple of 8 (got %d)", N);
+  TFIMM_CHECK_ARG(out_dtype == kBF16 || out_dtype == kF32, "conv: out_dtype must be bf16 or f32");
+  TFIMM_CHECK_ARG(bias == nullptr || (reinterpret_cast<uintptr_t>(bias) & 15u) == 0, "conv: bias must be 16-byte aligned");
+  const int Ho = (H + 2 * pad - ks) / stride + 1, Wo = (Wd + 2 * pad - ks) / stride + 1;
+  TFIMM_CHECK_ARG(Ho > 0 && Wo > 0, "conv: empty output");
+  GemmParams p{};
+  p.N = N; p.K = ks * ks * C;
+  p.bias = bias; p.act = act; p.has_res = residual != nullptr ? 1 : 0; p.act_post = act_post;
+  p.conv = 1; p.cv_cblocks = C / 64; p.cv_ks = ks; p.cv_stride = stride; p.cv_pad = pad;
+  // 128-pixel output patch: 8 x 16 pixels of one image, or 8 x 8 pixels of two images for small feature maps
+  if (Wo > 8) { p.cv_pb = 1; p.cv_ph = 8; p.cv_pw = 16; }
+  else { p.cv_pb = 2; p.cv_ph = 8; p.cv_pw = 8; }
+  p.cv_tiles_x = (Wo + p.cv_pw - 1) / p.cv_pw;
+  p.cv_tiles_y = (Ho + p.cv_ph - 1) / p.cv_ph;
+  const int tiles_b = (B + p.cv_pb - 1) / p.cv_pb;
+  p.M = tiles_b * p.cv_tiles_y * p.cv_tiles_x * kBlockM;  // padded row count: every tile is a full patch
+  const int bn = N >= 256 ? 256 : (N >= 128 ? 128 : 64);
+#define TFIMM_CONV_CASE(BN)                                                                                       \
+  case BN:                                                                                                        \
+    return out_dtype == kBF16                                                                                     \
+               ? launch_conv<BN, __nv_bfloat16>(x, W, ldw, residual, out, B, H, Wd, C, Ho, Wo, p, stream)           \
+               : launch_conv<BN, float>(x, W, ldw, residual, out, B, H, Wd, C, Ho, Wo, p, stream);
+  switch (bn) {
+    TFIMM_CONV_CASE(256)
+    TFIMM_CONV_CASE(128)
+    TFIMM_CONV_CASE(64)
+  }
+#undef TFIMM_CONV_CASE
+  return kInvalidArgument;
+}
+
+}  // namespace tfimm

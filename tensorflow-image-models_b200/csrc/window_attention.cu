@@ -1,6 +1,7 @@
 // Swin (shifted-)window attention on mma.sync, bf16, head_dim 32: tokens per window N <= 64, or N <= 144 (the 12 x 12
-// windows of the *_window12_384 models) in a second instantiation.  7 x 7 windows run on tcgen05
-// (window_attention_sm100.cu); this kernel covers the rest.
+// windows of the *_window12_384 models) in a second instantiation.  Two entry points share the kernel: one takes the
+// bias as [H][N][N] and the shift mask as per-token region labels, the other (kPadded, what the model uses for 7 x 7
+// windows) the bias as a padded [H][64][64] table and the mask as one 64-bit word per query row.
 //
 // Reference: WindowAttention.call (tfimm/architectures/swin.py:159-198) wrapped by
 // SwinTransformerBlock.call's tf.roll -> window_partition -> ... -> window_reverse -> tf.roll
@@ -25,12 +26,13 @@ __device__ __forceinline__ uint32_t wswz(int row, int chunk) {
   return (uint32_t)(row * 64 + ((chunk ^ ((row >> 1) & 3)) << 4));
 }
 
-template <int ROWS>   // padded tokens per window: 64 or 144
+template <int ROWS, bool kPadded>   // padded tokens per window: 64 or 144
 __global__ void __launch_bounds__(kWWarps * 32)
 window_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ out,
                              const float* __restrict__ bias, const int* __restrict__ row_map,
-                             const int* __restrict__ labels, long total_pairs, int nw_img, int N, int H,
-                             float scale) {
+                             const int* __restrict__ labels, const unsigned long long* __restrict__ maskbits,
+                             long total_pairs, int nw_img, int N, int H, float scale) {
+  static_assert(!kPadded || ROWS == 64, "the padded bias / mask-bit format is 64 x 64");
   constexpr int kWRows = ROWS;
   constexpr int kTileBytes = ROWS * kWDH * 2;   // 4 / 9 KB per q / k / v tile
   constexpr int NT = ROWS / 8;                  // key tiles of 8
@@ -67,7 +69,8 @@ window_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat1
   cp_async_commit();
 
   const int g = lane >> 2, t = lane & 3;
-  const float* bias_h = bias + (long)h * N * N;
+  const int bias_ld = kPadded ? 64 : N;
+  const float* bias_h = bias + (long)h * bias_ld * bias_ld;
   cp_async_wait<0>();
   __syncwarp();
 
@@ -109,8 +112,12 @@ window_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat1
         const int row = (e >> 1) ? r1 : r0;
         float val = -INFINITY;
         if (key < N && row < N) {
-          val = fmaf(s[nt][e], scale, __ldg(bias_h + (long)row * N + key));   // L1 / L2-resident table
-          if (labels != nullptr && s_lab[warp][key] != ((e >> 1) ? lab1 : lab0)) val += -100.0f;
+          val = fmaf(s[nt][e], scale, __ldg(bias_h + (long)row * bias_ld + key));   // L1 / L2-resident table
+          if constexpr (kPadded) {
+            if (maskbits != nullptr && ((__ldg(maskbits + wi * 64 + row) >> key) & 1ull)) val += -100.0f;
+          } else {
+            if (labels != nullptr && s_lab[warp][key] != ((e >> 1) ? lab1 : lab0)) val += -100.0f;
+          }
         } else if (key < N) {
           val = 0.f;  // padded query rows: keep finite, result is discarded
         }
@@ -176,6 +183,24 @@ window_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat1
   }
 }
 
+template <int ROWS, bool kPadded>
+int launch_window_attention(const void* qkv, void* out, const float* bias, const int* row_map, const int* labels,
+                            const unsigned long long* maskbits, int B, int nw_img, int N, int H, float scale,
+                            cudaStream_t stream) {
+  const long pairs = (long)B * nw_img * H;
+  const unsigned grid = (unsigned)((pairs + kWWarps - 1) / kWWarps);
+  constexpr int smem = kWWarps * 3 * ROWS * kWDH * 2;   // 48 KB / 108 KB (two CTAs per SM)
+  auto kernel = window_attention_bf16_kernel<ROWS, kPadded>;
+  static unsigned long long attr_devs = 0;
+  if (first_use_on_device(attr_devs))
+    TFIMM_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  kernel<<<grid, kWWarps * 32, smem, stream>>>(reinterpret_cast<const __nv_bfloat16*>(qkv),
+                                               reinterpret_cast<__nv_bfloat16*>(out), bias, row_map, labels, maskbits,
+                                               pairs, nw_img, N, H, scale);
+  TFIMM_LAUNCH_OK("window_attention_bf16_kernel");
+  return kOk;
+}
+
 }  // namespace
 
 int window_attention_bf16(const void* qkv, void* out, const float* bias, const int* row_map,
@@ -187,27 +212,28 @@ int window_attention_bf16(const void* qkv, void* out, const float* bias, const i
     set_last_error("window_attention: bf16 kernel supports head_dim 32 and <= 144 tokens per window (got dh=%d N=%d)", dh, N);
     return kUnsupported;
   }
-  const long pairs = (long)B * nw_img * H;
-  const unsigned grid = (unsigned)((pairs + kWWarps - 1) / kWWarps);
-  if (N <= 64) {
-    constexpr int smem = kWWarps * 3 * 64 * kWDH * 2;
-    static unsigned long long attr_devs = 0;
-    if (first_use_on_device(attr_devs))
-      TFIMM_CUDA_OK(cudaFuncSetAttribute(window_attention_bf16_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    window_attention_bf16_kernel<64><<<grid, kWWarps * 32, smem, stream>>>(
-        reinterpret_cast<const __nv_bfloat16*>(qkv), reinterpret_cast<__nv_bfloat16*>(out), bias, row_map, labels,
-        pairs, nw_img, N, H, scale);
-  } else {
-    constexpr int smem = kWWarps * 3 * 144 * kWDH * 2;   // 108 KB: two CTAs per SM
-    static unsigned long long attr_devs = 0;
-    if (first_use_on_device(attr_devs))
-      TFIMM_CUDA_OK(cudaFuncSetAttribute(window_attention_bf16_kernel<144>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    window_attention_bf16_kernel<144><<<grid, kWWarps * 32, smem, stream>>>(
-        reinterpret_cast<const __nv_bfloat16*>(qkv), reinterpret_cast<__nv_bfloat16*>(out), bias, row_map, labels,
-        pairs, nw_img, N, H, scale);
+  if (N <= 64)
+    return launch_window_attention<64, false>(qkv, out, bias, row_map, labels, nullptr, B, nw_img, N, H, scale, stream);
+  return launch_window_attention<144, false>(qkv, out, bias, row_map, labels, nullptr, B, nw_img, N, H, scale, stream);
+}
+
+// bias_pad: [H][64][64] fp32 (rows / columns beyond N are ignored); maskbits: [nw_img][64] uint64, bit j of entry
+// (wi, i) set when tokens i and j of window wi lie in different shift regions (null for unshifted blocks).
+int window_attention_tc_bf16(const void* qkv, void* out, const float* bias_pad, const int* row_map,
+                             const unsigned long long* maskbits, int B, int nw_img, int N, int H, int dh, float scale,
+                             cudaStream_t stream) {
+  TFIMM_CHECK_ARG(B > 0 && nw_img > 0 && N > 0 && H > 0, "window_attention: bad shape");
+  TFIMM_CHECK_ARG(bias_pad != nullptr && row_map != nullptr, "window_attention: bias and row_map are required");
+  if (dh != kWDH || N > 52) {
+    set_last_error("window_attention: the padded-table entry takes head_dim 32 and <= 52 tokens per window (got dh=%d N=%d)",
+                   dh, N);
+    return kUnsupported;
   }
-  TFIMM_LAUNCH_OK("window_attention_bf16_kernel");
-  return kOk;
+  TFIMM_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15u) == 0 && (reinterpret_cast<uintptr_t>(out) & 15u) == 0 &&
+                      (reinterpret_cast<uintptr_t>(bias_pad) & 15u) == 0,
+                  "window_attention: qkv / out / bias must be 16-byte aligned");
+  return launch_window_attention<64, true>(qkv, out, bias_pad, row_map, nullptr, maskbits, B, nw_img, N, H, scale,
+                                           stream);
 }
 
 }  // namespace tfimm

@@ -1,4 +1,4 @@
-"""tfimm_b200: a B200-native (sm_100a) inference engine behind tfimm's public API.
+"""tfimm_b200: a H100-native (sm_90a) inference engine behind tfimm's public API.
 
 Drop-in for the image-classifier forward path of martinsbruveris/tensorflow-image-models
 (reference ``tfimm/__init__.py:1-12``): ``create_model``, ``create_preprocessing``,

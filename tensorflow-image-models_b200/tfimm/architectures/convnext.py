@@ -1,4 +1,4 @@
-"""ConvNeXt forward path as a chain of sm_100a kernels.
+"""ConvNeXt forward path as a chain of sm_90a kernels.
 
 What the reference computes (tfimm/architectures/convnext.py):
   stem Conv2D(k = s = patch) + LN -> 4 stages; stage s>0 starts with LN + Conv2D(k = s = 2);
@@ -6,10 +6,10 @@ What the reference computes (tfimm/architectures/convnext.py):
   head: global average pool -> LN -> Dense                              [convnext.py:219-228, 286-295, 375-440]
 
 How it runs here:
-  stem: patchify gather + tcgen05 GEMM (K = 48) + LN into the residual stream
-  downsample: ONE kernel does LN per pixel and writes the 2x2 im2col layout, then a tcgen05 GEMM
+  stem: patchify gather + wgmma GEMM (K = 48) + LN into the residual stream
+  downsample: ONE kernel does LN per pixel and writes the 2x2 im2col layout, then a wgmma GEMM
   block: [dw7x7 + bias + LN] (one CUDA-core kernel, bf16 out) -> [fc1 + bias + GELU] ->
-         [fc2 + bias, * gamma, + shortcut, in place]   (the last two are the tcgen05 GEMM epilogues)
+         [fc2 + bias, * gamma, + shortcut, in place]   (the last two are the wgmma GEMM epilogues)
   head: pool kernel -> LN -> GEMM
 """
 import os
@@ -158,7 +158,7 @@ class ConvNeXt(Model):
             for k, blk in enumerate(st["blocks"]):
                 h = ops.dwconv_ln(xs.view(B, H, W, dim), blk["dw_w"], blk["dw_b"], *blk["n"], eps, adt)
                 if adt == torch.bfloat16 and ops.mlp_fused_supported(dim, blk["fc1_w"].shape[0]):
-                    # one kernel: the (M, 4 dim) hidden activations stay in tensor memory (csrc/mlp_sm100.cu)
+                    # one kernel: the (M, 4 dim) hidden activations stay on the SM (csrc/mlp_sm90.cu)
                     ops.mlp_fused(h.view(-1, dim), blk["fc1_w"], blk["fc1_b"], blk["fc2_w"], blk["fc2_b"], c.act_layer,
                                   gamma=blk["ls"], residual=xs, out=xs)
                 else:

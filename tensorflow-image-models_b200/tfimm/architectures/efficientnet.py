@@ -1,4 +1,4 @@
-"""EfficientNet / MobileNet-V2 family forward path as a chain of sm_100a kernels.
+"""EfficientNet / MobileNet-V2 family forward path as a chain of sm_90a kernels.
 
 What the reference computes (tfimm/architectures/efficientnet.py, efficientnet_blocks.py,
 efficientnet_builder.py): stem Conv3x3/s2 + BN + act -> stages of MBConv-style blocks decoded from
@@ -6,11 +6,11 @@ strings such as ``ir_r2_k3_s2_e6_c24_se0.25`` -> 1x1 head conv + BN + act -> glo
                                                    [efficientnet.py:278-345, efficientnet_blocks.py:348-535]
 
 How it runs here (inference, so every BatchNorm is folded into the preceding conv at load time):
-  1x1 convs (expand / project / head)   tcgen05 GEMM, folded-BN bias + act (+ residual) in the epilogue
+  1x1 convs (expand / project / head)   wgmma GEMM, folded-BN bias + act (+ residual) in the epilogue
   depthwise k x k (TF "same" or symmetric pad)  one CUDA-core kernel with bias + act and the squeeze
                                                 (per-image channel sums) fused in
   squeeze-excite                        one tiny kernel per block for the two FCs + a channel-scale pass
-  dense k x k convs (stem, fused-MBConv) im2col gather + tcgen05 GEMM
+  dense k x k convs (stem, fused-MBConv) im2col gather + wgmma GEMM
 """
 import math
 import re
@@ -331,9 +331,7 @@ class EfficientNet(Model):
 
     def _project(self, h, wb, act, shortcut, gate):
         """1 x 1 projection after the (optional) squeeze-excite gate.  With >= 256 pixels per image the gate is applied
-        inside the GEMM (measured on B200, batch 256: 287 vs 489 us at 95 x 95 x 144 -> 32, 73 vs 118 us at 24 x 24 x 672
-        -> 112).  Small feature maps -- a 128-row tile spans several images, long contractions: 176 vs 118 us at
-        12 x 12 x 1632 -> 272 -- keep the separate pass."""
+        inside the GEMM.  Small feature maps (a 128-row tile spans several images) keep the separate pass."""
         if gate is not None and (h.dtype != torch.bfloat16 or h.shape[1] * h.shape[2] < 256):
             h, gate = ops.scale_channels_(h, gate), None
         return self._dense_conv(h, wb, 1, 1, act, residual=shortcut, gate=gate)

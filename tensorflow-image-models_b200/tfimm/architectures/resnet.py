@@ -1,13 +1,13 @@
-"""ResNet / ResNeXt / SE-ResNet / ECA-ResNet forward path as a chain of sm_100a kernels.
+"""ResNet / ResNeXt / SE-ResNet / ECA-ResNet forward path as a chain of sm_90a kernels.
 
 What the reference computes (tfimm/architectures/resnet.py): stem (7x7/s2 conv or three 3x3 convs) + BN
 + ReLU -> 3x3/s2 max-pool (or conv) -> 4 stages of BasicBlock / Bottleneck with projection shortcuts
 (conv or avg-pool + 1x1) -> global average pool -> Dense.          [resnet.py:166-189, 266-292, 295-382, 466-593]
 
 How it runs here (BatchNorm folded into the preceding conv at load time):
-  1x1 convs                   tcgen05 GEMM; the last conv of a block adds the shortcut and applies the
+  1x1 convs                   wgmma GEMM; the last conv of a block adds the shortcut and applies the
                               ReLU in its epilogue (act_after_residual)
-  3x3 / 7x7 dense convs       im2col gather + tcgen05 GEMM
+  3x3 / 7x7 dense convs       im2col gather + wgmma GEMM
   grouped 3x3 (ResNeXt)       CUDA-core grouped-conv kernel (4..32 channels per group)
   SE / ECA                    pool + tiny gate kernel, then one fused  x = relu(x * gate + shortcut)  pass
 Not implemented (raise at construction): BlurPool anti-aliasing (1 registration), GroupNorm (1), groups
@@ -136,7 +136,7 @@ class ResNet(Model):
         if isinstance(cfg, dict):
             cfg = ResNetConfig(**cfg)
         if cfg.norm_layer not in _BN_EPS and cfg.norm_layer not in _GN_GROUPS:
-            raise NotImplementedError(f"norm_layer={cfg.norm_layer} is not implemented in the B200 engine.")
+            raise NotImplementedError(f"norm_layer={cfg.norm_layer} is not implemented in this engine.")
         if cfg.aa_layer not in ("", "blur_pool"):
             raise ValueError(f"Unknown anti-aliasing layer {cfg.aa_layer}")
         if cfg.attn_layer not in ("", "se", "eca"):

@@ -1,4 +1,4 @@
-"""Swin Transformer forward path as a chain of sm_100a kernels.
+"""Swin Transformer forward path as a chain of sm_90a kernels.
 
 What the reference computes (tfimm/architectures/swin.py): PatchEmbeddings(k = s = 4) + LN -> 4 stages of
 SwinTransformerBlocks [LN -> roll(-s) -> window_partition -> WindowAttention(+rel-pos bias, +shift mask)
@@ -9,7 +9,7 @@ How it runs here: tokens stay in raster order for the whole network.  The two ro
 and the reverse are row permutations, so they are folded into a row-index table consumed by the
 window-attention kernel (gather q/k/v rows, scatter output rows); the shift mask is regenerated
 from per-token region labels; PatchMerging's strided gather + concat is fused with its LayerNorm.
-GEMMs (qkv / proj / fc1 / fc2 / reduction / head) run on tcgen05 with bias / GELU / residual epilogues.
+GEMMs (qkv / proj / fc1 / fc2 / reduction / head) run on wgmma with bias / GELU / residual epilogues.
 """
 from collections import OrderedDict
 from dataclasses import dataclass
@@ -249,7 +249,7 @@ class SwinTransformer(Model):
                 table = self.params[f"{p}/attn/relative_position_bias_table"].float()
                 bias = table[index].view(n, n, heads).permute(2, 0, 1).contiguous()  # tf.gather + transpose
                 bias_pad = None
-                if n <= 52:  # tcgen05 window-attention kernel: 16-byte aligned rows of 64
+                if n <= 52:  # padded-table window-attention entry: 16-byte aligned rows of 64
                     bias_pad = torch.zeros((heads, 64, 64), device=dev, dtype=torch.float32)
                     bias_pad[:, :n, :n] = bias
                 st["blocks"].append(dict(
@@ -317,7 +317,7 @@ class SwinTransformer(Model):
                 ops.gemm(a, blk["proj_w"], bias=blk["proj_b"], residual=xs, out=xs)
                 t = ops.layernorm(xs, *blk["n2"], eps, adt)
                 if adt == torch.bfloat16 and ops.mlp_fused_supported(dim, blk["fc1_w"].shape[0]):
-                    # one kernel: the (M, 4 dim) hidden activations stay in tensor memory (csrc/mlp_sm100.cu)
+                    # one kernel: the (M, 4 dim) hidden activations stay on the SM (csrc/mlp_sm90.cu)
                     ops.mlp_fused(t, blk["fc1_w"], blk["fc1_b"], blk["fc2_w"], blk["fc2_b"], c.act_layer, residual=xs,
                                   out=xs)
                 else:

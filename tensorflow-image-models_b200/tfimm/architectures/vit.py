@@ -1,4 +1,4 @@
-"""ViT / DeiT forward path as a chain of sm_100a kernels.
+"""ViT / DeiT forward path as a chain of sm_90a kernels.
 
 What the reference computes (tfimm/architectures/vit.py): PatchEmbeddings conv (k = s = patch)
 -> prepend cls (and dist) token -> + pos_embed -> nb_blocks x [x + attn(LN(x)); x + mlp(LN(x))]
@@ -7,7 +7,7 @@ What the reference computes (tfimm/architectures/vit.py): PatchEmbeddings conv (
 
 How it runs here (per image batch, all on the current CUDA stream):
   patchify (im2col gather, fp32/bf16/u8 in -> bf16)            1 kernel
-  patch GEMM + bias (tcgen05)                                  1 kernel
+  patch GEMM + bias (wgmma)                                  1 kernel
   assemble tokens (+cls, +pos) into the fp32 residual stream   1 kernel
   per block: LN -> qkv GEMM -> fused attention -> proj GEMM(+residual, in place)
              LN -> fc1 GEMM(+GELU) -> fc2 GEMM(+residual, in place)          7 kernels

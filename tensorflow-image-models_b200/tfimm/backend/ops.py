@@ -91,7 +91,7 @@ def act_code(act) -> int:
 def gemm(a, w, bias=None, act=None, gamma=None, residual=None, out=None, out_dtype=None, block_n=0,
          act_after_residual=False):
     """out = residual + gamma * act(a @ w.T + bias)  (act_after_residual: act(residual + gamma*(...))).
-    a:(M,K), w:(N,K); bf16 -> tcgen05, fp32 -> SIMT."""
+    a:(M,K), w:(N,K); bf16 -> wgmma, fp32 -> SIMT."""
     _cuda(a, w, bias, gamma, residual, out)
     M, K = a.shape
     N = w.shape[0]
@@ -142,7 +142,7 @@ def gemm_gated(a, gate, rows_per_image, w, bias=None, act=None, residual=None):
 
 
 def mlp_fused_supported(C, hidden):
-    """Shapes of the fused fc1 -> act -> fc2 kernel (csrc/mlp_sm100.cu)."""
+    """Shapes of the fused fc1 -> act -> fc2 kernel (csrc/mlp_sm90.cu)."""
     return C in (96, 128, 192, 256) and hidden % 128 == 0 and hidden >= 256
 
 
@@ -361,7 +361,7 @@ def window_attention(qkv, bias, row_map, labels, B, nw_img, N, H, dh, scale):
 
 
 def window_attention_tc(qkv, bias_pad, row_map, maskbits, B, nw_img, N, H, dh, scale):
-    """Swin (shifted-)window attention on tcgen05 (head_dim 32, N <= 52): token-ordered qkv (B*nw_img*N, 3*H*dh) ->
+    """Swin (shifted-)window attention for 7 x 7 windows (head_dim 32, N <= 52): token-ordered qkv (B*nw_img*N, 3*H*dh) ->
     (B*nw_img*N, H*dh).  bias_pad: fp32 (H, 64, 64); maskbits: int64 (nw_img, 64) or None (see window_mask_bits)."""
     _cuda(qkv, bias_pad, row_map, maskbits)
     assert qkv.shape == (B * nw_img * N, 3 * H * dh) and qkv.is_contiguous() and qkv.dtype == torch.bfloat16

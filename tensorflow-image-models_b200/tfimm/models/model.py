@@ -10,7 +10,7 @@ Contract kept from the reference (SURVEY.md 8b; e.g. tfimm/architectures/vit.py:
     flat ``{path: array}`` dict converted by the reference's own rules loads unchanged.
 
 What is different by design: weights live in HBM as torch CUDA tensors; the forward pass is a
-sequence of hand-written sm_100a kernels (tfimm.backend.ops); inference only.
+sequence of hand-written sm_90a kernels (tfimm.backend.ops); inference only.
 """
 import math
 from collections import OrderedDict
@@ -201,7 +201,7 @@ class Model:
     def _ensure_plan(self):
         if self.device.type != "cuda":
             raise _lib.KernelLibraryError(
-                "tfimm_b200 models only run on a CUDA device (sm_100a); there is no CPU fallback. "
+                "tfimm_b200 models only run on a CUDA device (sm_90a); there is no CPU fallback. "
                 "The model was created on device '%s'." % self.device
             )
         if self._plan is None:
@@ -275,7 +275,7 @@ class Model:
         """Captures one forward pass (fixed batch / input size) into a CUDA graph and returns a callable
         ``f(x) -> logits`` that copies ``x`` into the graph's static input and replays it: the ~90-400 kernel
         launches of a forward become one graph launch, which removes the host-side launch gaps (this is the
-        B200-native replacement for the reference's ``tf.function(jit_compile=True)`` wrapper,
+        H100-native replacement for the reference's ``tf.function(jit_compile=True)`` wrapper,
         tfimm/utils/profile.py:88-90).  The returned tensor is overwritten by the next call."""
         from ..backend import ops
 

@@ -1,6 +1,6 @@
 """Shared pytest configuration.
 
-* registers the ``gpu`` marker (tests that need a B200; the driver runs ``-m gpu`` on the box)
+* registers the ``gpu`` marker (tests that need an H100; select them with ``-m gpu``)
 * puts the in-tree package (``tensorflow-image-models_b200/``) and the repo root on sys.path
 * makes sure the CUDA library is built (nvcc cross-compiles here without a GPU)
 """
@@ -18,7 +18,7 @@ for p in (str(ROOT), str(PKG)):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (B200); run with -m gpu")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (H100); run with -m gpu")
 
 
 def pytest_collection_modifyitems(config, items):

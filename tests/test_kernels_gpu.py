@@ -243,9 +243,9 @@ def test_attention_bf16(B, N, H):
     err = (out.float() - ref).abs().max().item()
     assert err < 3e-2, err   # P is rounded to bf16 before the PV product; output rounded to bf16
     if N <= 256:
-        # tcgen05 kernel vs the emulation that rounds P the same way (global row max): only the output rounding
-        # (2^-9 relative) remains.  The resident-KV kernel for longer sequences rounds P per 64-key block of its
-        # online softmax, so it is only held to the bound above.
+        # vs the emulation that rounds P with the global row max: at these lengths the kernel's per-64-key-block
+        # rounding of P in its online softmax stays within the output rounding (2^-9 relative) of it.  Longer
+        # sequences are only held to the bound above.
         from oracle import emulate_bf16
         emu = emulate_bf16.attention(qkv, B, N, H, dh, dh ** -0.5).float()
         assert (out.float() - emu).abs().max().item() < 2.0 ** -8 * emu.abs().max().item() + 1e-6
@@ -421,7 +421,7 @@ def test_window_attention_bf16(h, w, ws, shift, H):
     ref = torch.roll(ow, (shift, shift), (1, 2)).reshape(B * h * w, C)
     err = (out.float() - ref).abs().max().item()
     assert err < 3e-2, err
-    # tcgen05 kernel (two windows per UMMA tile): padded bias table + per-row 64-bit region masks
+    # padded-table entry point: padded bias table + per-row 64-bit region masks
     if n <= 52:
         bias_pad = torch.zeros(H, 64, 64, device="cuda")
         bias_pad[:, :n, :n] = bias
@@ -721,7 +721,7 @@ def test_gemm_short_contraction_streaming_kernel(M, K, N, act):
     assert out.shape == (M, N) and out.dtype == torch.bfloat16
     assert (out.float() - ref).abs().max().item() <= 2.0 ** -7 * ref.abs().max().item() + 1e-5
     assert (out != ref.to(torch.bfloat16)).float().mean().item() < 2e-2
-    # the tcgen05 path gives the same numbers (forced through block_n)
+    # the wgmma path gives the same numbers (forced through block_n)
     out2 = ops.gemm(a, w, bias=bias, act=act, block_n=64)
     assert (out.float() - out2.float()).abs().max().item() <= 2.0 ** -7 * ref.abs().max().item() + 1e-5
     # bf16 residual, also in place
@@ -792,7 +792,7 @@ def test_mlp_fused_rejects_other_shapes():
                                       (2, 36100, 32, 16), (5, 1000, 56, 336)])
 @pytest.mark.parametrize("with_res", [False, True])
 def test_gemm_gated_equals_scale_then_gemm(B, HW, K, N, with_res):
-    """Squeeze-excite gate applied to the A tile in shared memory (tcgen05 kernel) or to the A fragments in registers
+    """Squeeze-excite gate applied to the A tile in shared memory (wgmma kernel) or to the A fragments in registers
     (K <= 64: streaming kernel): the products scale_channels_ would have written, then the same GEMM."""
     ops = _ops()
     M = B * HW

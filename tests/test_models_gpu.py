@@ -2,10 +2,10 @@
 
 Error metric is the reference's own (tests/test_timm.py:71): max|a-b| / (max|b| + 1e-6); plain
 max|a-b| is printed next to it.  Tolerances:
-  * precision="fp32": 1e-5, north_star's own bound (measured on B200: 0.3-2e-6)
+  * precision="fp32": 1e-5, north_star's own bound (measured: 0.3-2e-6)
   * precision="bf16": north_star asks 1e-3, which no implementation that STORES activations in bf16 can meet (the
     ideal one -- exact arithmetic, same storage points -- is 3-7e-3 from the fp32 reference, see
-    tests/test_parity_budget_gpu.py).  Asserted here: ~1.3x the value measured on B200 for each family, so that a
+    tests/test_parity_budget_gpu.py).  Asserted here: ~1.3x the measured value for each family, so that a
     regression shows: ViT / Swin 1e-2 (measured 5-7e-3), ConvNeXt 7e-3 (4.5e-3), BN families 8e-3 (3-4e-3).
 """
 import pytest

@@ -7,7 +7,7 @@ lifts that guard for itself only.
 
 fp32 models (no bf16 storage anywhere) must reproduce the oracle to 1e-5; bf16 models exercise the bf16-only branches
 (fused MLP, gate inside the projection GEMM, tensor-core window attention tables) and must land within the bf16 error
-budget measured on B200 (DESIGN.md section 5).
+budget measured in tests/test_parity_budget_gpu.py.
 """
 import importlib
 

@@ -1,13 +1,13 @@
 """bf16 parity as a MEASURED BUDGET (VERDICT r01 item 1).
 
-north_star: logits within 1e-3 (bf16) / 1e-5 (fp32) of the reference.  What is tested, and what was learned on B200:
+north_star: logits within 1e-3 (bf16) / 1e-5 (fp32) of the reference.  What is tested, and what was learned:
 
 A. ``engine(fp32 mode)`` vs the oracle / the reference-generated logits <= 1e-5      (here, full size, and
    tests/test_models_gpu.py).
 D. The emulation graph (``oracle/emulate_bf16``: the engine's orchestration on exact float64 torch ops) with no bf16
    storage anywhere reproduces the oracle -- which is pinned to the reference's own code
    (tests/test_reference_pin_cpu.py) -- so the comparisons below are against the reference's graph.
-C. ``engine(bf16)`` vs fp32 oracle: the total error, asserted at ~1.3x the value measured on B200.
+C. ``engine(bf16)`` vs fp32 oracle: the total error, asserted at ~1.3x the measured value.
 B. ``engine(bf16)`` vs the emulation WITH THE SAME bf16 STORAGE POINTS.  The judge asked for <= 1e-3 here.  Measured:
    2-3e-3 -- and so is the distance between TWO EXACT emulations that differ only in float64 vs float32 arithmetic
    (the "divergence floor").  bf16 storage is chaotic at this level: a 1e-7 perturbation flips the rounding of a few
@@ -86,7 +86,7 @@ def _rms(a, b):
     return ((a.double() - b.double()).pow(2).mean().sqrt() / b.double().pow(2).mean().sqrt()).item()
 
 
-# (family, model, overrides, batch, bound on C = ~1.3 x the max-norm error measured on B200)
+# (family, model, overrides, batch, bound on C = ~1.3 x the max-norm error measured)
 BUDGET = [
     ("vit", "vit_tiny_patch16_224", {}, 8, 8e-3),
     ("vit", "vit_base_patch16_224", {}, 4, 8e-3),
