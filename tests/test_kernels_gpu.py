@@ -9,6 +9,8 @@ import math
 import pytest
 import torch
 
+from oracle.shadow import faithful
+
 pytestmark = pytest.mark.gpu
 
 
@@ -71,9 +73,9 @@ def test_gemm_bf16_plain(M, N, K, out_dtype):
 @pytest.mark.parametrize("M,N,K", [(256, 256, 64), (512, 768, 768), (394, 2304, 768), (1000, 1000, 1024),
                                    (50432 // 4, 768, 3072), (300, 384, 128), (77, 1000, 192), (4736, 3072, 768)])
 @pytest.mark.parametrize("out_dtype", [torch.bfloat16, torch.float32])
-def test_gemm_bf16_cta_pair(M, N, K, out_dtype):
-    """block_n=2 forces the cta_group::2 kernel (256x256 tiles over two SMs): M/N tails, many tiles per pair
-    (accumulator-stage and smem-ring wrap-around), residual in place."""
+def test_gemm_bf16_256_wide_tile(M, N, K, out_dtype):
+    """block_n=2 (an alias of block_n=256) forces the 256-wide tile: M/N tails, many tiles per grid (smem-ring and
+    mbarrier-phase wrap-around), residual in place."""
     ops = _ops()
     g = torch.Generator(device="cuda").manual_seed(M * 7 + N * 3 + K)
     a = torch.randn(M, K, device="cuda", generator=g).to(torch.bfloat16)
@@ -668,22 +670,10 @@ def test_gemm_activation_epilogue_is_faithfully_rounded(act, block_n):
     torch.cuda.synchronize()
     y = a.double() @ w.double().t() + bias.double()
     ref = 0.5 * y * (1.0 + torch.erf(y / 2.0 ** 0.5)) if act == "gelu" else y * torch.sigmoid(y)
-    flips, worst = _faithful(out, ref)
+    flips, worst = faithful(out, ref)
     print(f"{act} block_n={block_n}: {100 * flips:.3f}% of the bf16 outputs (|y| >= 0.05) differ from the correct rounding, "
           f"worst error {worst:.3f} x max(bf16 spacing, 5e-6)")
     assert flips < 2e-2 and worst <= 1.0
-
-
-def _faithful(out, ref):
-    """(fraction of outputs with |ref| >= 0.05 that are not the correctly rounded bf16 value, worst error in units of
-    max(one bf16 spacing at that magnitude, 5e-6)).  Below ~1e-3 in magnitude an output's own ulp is smaller than the
-    4e-6 absolute accuracy of the activation polynomials -- and irrelevant to the next layer's sums."""
-    want = ref.to(torch.bfloat16)
-    big = ref.abs() >= 0.05
-    flips = ((out != want) & big).float().sum().item() / max(big.float().sum().item(), 1.0)
-    unit = torch.maximum(ref.abs() * 2.0 ** -7, torch.full_like(ref, 5e-6))
-    worst = ((out.double() - ref).abs() / unit).max().item()
-    return flips, worst
 
 
 def test_dwconv_swish_is_faithfully_rounded():
@@ -698,7 +688,7 @@ def test_dwconv_swish_is_faithfully_rounded():
     wt = wgt.double().view(3, 3, C).permute(2, 0, 1)[:, None]
     y = torch.nn.functional.conv2d(x.double().permute(0, 3, 1, 2), wt, bias.double(), padding=1, groups=C).permute(0, 2, 3, 1)
     ref = y * torch.sigmoid(y)
-    flips, worst = _faithful(out, ref)
+    flips, worst = faithful(out, ref)
     print(f"dwconv swish: {100 * flips:.3f}% flips, worst {worst:.3f} x max(bf16 spacing, 5e-6)")
     assert flips < 2e-2 and worst <= 1.0
 
@@ -741,7 +731,7 @@ def test_gemm_short_contraction_streaming_kernel(M, K, N, act):
                                       (80 * 256 + 3, 192, 4), (1024, 192, 2)])
 @pytest.mark.parametrize("act,with_gamma", [("gelu", True), ("gelu", False), ("swish", False)])
 def test_mlp_fused_equals_two_gemms(M, C, mult, act, with_gamma):
-    """fc1 -> act -> fc2 -> * gamma -> + residual in one kernel (csrc/mlp_sm100.cu): same rounding points as the
+    """fc1 -> act -> fc2 -> * gamma -> + residual in one kernel (csrc/mlp_sm90.cu): same rounding points as the
     two-GEMM form (bf16 hidden, fp32 accumulation in ascending k), so the two agree to fp32 summation noise."""
     ops = _ops()
     Hd = mult * C

@@ -21,7 +21,7 @@ B. ``engine(bf16)`` vs the emulation WITH THE SAME bf16 STORAGE POINTS.  The jud
          is the correctly rounded value or its neighbour).
 
 Also here: the BASELINE.json configurations at their OWN batch size (256 per GPU) through ``model.cuda_graph`` -- the
-CTA-pair GEMM, the persistent multi-wave attention schedule, the pruned last ViT block and graph replay, which the
+256-wide GEMM tile, the persistent multi-wave attention schedule, the pruned last ViT block and graph replay, which the
 batch-2 tests never reach.
 """
 import importlib
