@@ -103,6 +103,28 @@ int tfimm_b200_gemm_f32(const float* A, int lda, const float* W, int ldw, const 
                         const float* gamma, const float* residual, int ldr, float* C, int ldc, int M, int N,
                         int K, int act, int act_after_residual, void* stream);
 
+/* precision="tf32": fp32 storage, TF32 tensor-core products (TensorFlow's default for fp32 matmuls and convolutions
+ * on Ampere and newer GPUs).  Same contract as tfimm_b200_gemm_bf16 with A, W, C, residual all fp32; the kernel rounds
+ * every A element to TF32 (round to nearest, ties away from zero: cvt.rna.tf32.f32) in shared memory before the
+ * product and accumulates in fp32; bias, activation, gamma and residual are applied in fp32.
+ * PRECONDITION: W must already be TF32-representable (the low 13 bits of every element zero), i.e. rounded the same way
+ * once, when the weights are prepared; the kernel does not round W.  K % 4 == 0; A, W, C, residual 16-byte aligned with
+ * row strides of a multiple of 16 bytes.  force_block_n: 0 = auto; 64 / 128 = that tile width; 2 = the widest (128). */
+int tfimm_b200_gemm_tf32(const float* A, int lda, const float* W, int ldw, const float* bias, const float* gamma,
+                         const float* residual, int ldr, float* C, int ldc, int M, int N, int K, int act,
+                         int act_after_residual, int force_block_n, void* stream);
+
+/* Implicit k x k convolution of tfimm_b200_conv_bf16 in fp32 with TF32 products: x NHWC fp32 with C % 32 == 0,
+ * W fp32 [N][k*k*C] (TF32-representable, as for tfimm_b200_gemm_tf32), out / residual NHWC fp32. */
+int tfimm_b200_conv_tf32(const float* x, const float* W, int ldw, const float* bias, const float* residual, float* out,
+                         int B, int H, int Wd, int C, int N, int ks, int stride, int pad, int act,
+                         int act_after_residual, void* stream);
+
+/* ViT self-attention of tfimm_b200_attention_bf16 on fp32 qkv / out with TF32 products: q, k, v rounded to TF32
+ * (cvt.rna) as they are loaded, fp32 online softmax, P rounded to TF32 before P V, fp32 accumulation.  K / V stream
+ * through shared memory in 64-key blocks, so N is not limited.  dh == 64 (other head dims: TFIMM_B200_UNSUPPORTED). */
+int tfimm_b200_attention_tf32(const float* qkv, float* out, int B, int N, int H, int dh, float scale, void* stream);
+
 /* LayerNorm over the last axis, fp32 statistics (tfimm/layers/factory.py:37-45).
  * in_stride/out_stride in elements (lets the caller normalise only token 0 of each image:
  * tfimm/architectures/vit.py:452,462). */

@@ -48,6 +48,11 @@ int conv_bf16_dispatch(const void*, const void*, int, const float*, const void*,
                        int, int, int, int, int, cudaStream_t);
 int gemm_f32(const float*, int, const float*, int, const float*, const float*, const float*, int, float*, int,
              int, int, int, int, int, cudaStream_t);
+int gemm_tf32_dispatch(const float*, int, const float*, int, const float*, const float*, const float*, int, float*, int,
+                       int, int, int, int, int, int, cudaStream_t);
+int conv_tf32_dispatch(const float*, const float*, int, const float*, const float*, float*, int, int, int, int, int, int,
+                       int, int, int, int, cudaStream_t);
+int attention_tf32(const float*, float*, int, int, int, int, float, cudaStream_t);
 int layernorm_rows(const void*, int, long, const float*, const float*, void*, int, long, long, int, float,
                    cudaStream_t);
 int layernorm_patch2x2(const void*, int, const float*, const float*, void*, int, int, int, int, int, float,
@@ -124,6 +129,24 @@ int tfimm_b200_gemm_f32(const float* A, int lda, const float* W, int ldw, const 
                         int act_after_residual, void* stream) {
   return tfimm::gemm_f32(A, lda, W, ldw, bias, gamma, residual, ldr, C, ldc, M, N, K, act, act_after_residual,
                          S(stream));
+}
+
+int tfimm_b200_gemm_tf32(const float* A, int lda, const float* W, int ldw, const float* bias, const float* gamma,
+                         const float* residual, int ldr, float* C, int ldc, int M, int N, int K, int act,
+                         int act_after_residual, int force_block_n, void* stream) {
+  return tfimm::gemm_tf32_dispatch(A, lda, W, ldw, bias, gamma, residual, ldr, C, ldc, M, N, K, act, act_after_residual,
+                                   force_block_n, S(stream));
+}
+
+int tfimm_b200_conv_tf32(const float* x, const float* W, int ldw, const float* bias, const float* residual, float* out,
+                         int B, int H, int Wd, int C, int N, int ks, int stride, int pad, int act,
+                         int act_after_residual, void* stream) {
+  return tfimm::conv_tf32_dispatch(x, W, ldw, bias, residual, out, B, H, Wd, C, N, ks, stride, pad, act,
+                                   act_after_residual, S(stream));
+}
+
+int tfimm_b200_attention_tf32(const float* qkv, float* out, int B, int N, int H, int dh, float scale, void* stream) {
+  return tfimm::attention_tf32(qkv, out, B, N, H, dh, scale, S(stream));
 }
 
 int tfimm_b200_layernorm(const void* x, int in_dtype, long in_stride, const float* gamma, const float* beta,

@@ -11,7 +11,10 @@
 // query tiles and runs a flash-style online softmax over 64-key blocks with
 // mma.sync m16n8k16 (fp32 accumulate, fp32 softmax statistics).
 //
-// fp32 path (precision="fp32" parity mode): plain SIMT, one warp per query row.
+// tf32 path (precision="tf32"): fp32 qkv / out, mma.sync m16n8k8 TF32, K / V streamed in 64-key blocks.
+//
+// fp32 path (precision="fp32" parity mode, and every call with bias / mask / probs / row_map): plain SIMT, one warp
+// per query row.
 #include "common.cuh"
 
 #include <stdlib.h>
@@ -209,6 +212,168 @@ int launch_vit_attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, in
   return kOk;
 }
 
+// ---- TF32 path (precision="tf32"): fp32 qkv / out, TF32 tensor-core products ----
+// One CTA per (image, head, 128-query chunk), 8 warps of 16 query rows.  fp32 K / V of a whole head do not fit shared
+// memory at N = 577 (295 KB), so they stream through a double-buffered cp.async ring of 64-key blocks shared by the
+// warps; each warp runs the flash-style online softmax of the bf16 kernel (fp32 statistics, exp2) with mma.sync
+// m16n8k8 TF32.  Q, K, V are rounded to TF32 (cvt.rna) as their fragments are loaded; P is rounded before PV.
+//
+// Fragment bookkeeping: the contraction index of an m16n8k8 product is free to permute as long as A and B agree.
+//   S = Q K^T: k-step ks covers dims 8 ks .. 8 ks + 7; logical k = t <-> dim 8 ks + 2t, k = t + 4 <-> dim 8 ks + 2t + 1,
+//              so each thread's two A (and two B) values are adjacent in memory: one 8-byte load.
+//   O = P V:   key tile nt; logical k = t <-> key 8 nt + 2t, k = t + 4 <-> key 8 nt + 2t + 1 -- exactly the two P values
+//              thread t holds in the S accumulator layout (columns 2t, 2t + 1), so P never moves between threads.
+// Row strides in shared memory: Q and K 72 floats (the 8-byte loads of a half-warp hit 32 distinct banks), V 68 floats
+// (rows 2t and 2t + 1 of the four t's land on distinct banks for each of the eight columns g).
+constexpr int kTfWarps = 8;
+constexpr int kTfRows = kTfWarps * 16;
+constexpr int kTfKeys = 64;
+constexpr int kTfLdK = 72, kTfLdV = 68;
+constexpr int kTfStageFloats = kTfKeys * (kTfLdK + kTfLdV);
+constexpr size_t kTfSmemBytes = (2 * kTfStageFloats + kTfRows * kTfLdK) * sizeof(float);   // K/V ring + Q: 106 KB
+
+__global__ void __launch_bounds__(kTfWarps * 32, 2)
+vit_attention_tf32_kernel(const float* __restrict__ qkv, float* __restrict__ out, int N, int H, float scale_log2) {
+  extern __shared__ __align__(16) float tsm[];
+  const int b = blockIdx.z, h = blockIdx.y;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int g = lane >> 2, t = lane & 3;
+  const long ld = 3L * H * kDH;
+  const float* base = qkv + (long)b * N * ld + h * kDH;
+  const int nblocks = (N + kTfKeys - 1) / kTfKeys;
+
+  // K / V block kb -> stage kb & 1 (16-byte chunks; keys >= N are zero-filled and masked below)
+  auto load_block = [&](int kb) {
+    float* sK = tsm + (kb & 1) * kTfStageFloats;
+    float* sV = sK + kTfKeys * kTfLdK;
+    for (int idx = tid; idx < kTfKeys * (kDH / 4); idx += kTfWarps * 32) {
+      const int r = idx >> 4, c = idx & 15;
+      const int key = kb * kTfKeys + r;
+      const bool valid = key < N;
+      const float* src = base + (long)(valid ? key : 0) * ld + c * 4;
+      cp_async_16(smem_u32(sK + r * kTfLdK + c * 4), src + H * kDH, valid);
+      cp_async_16(smem_u32(sV + r * kTfLdV + c * 4), src + 2 * H * kDH, valid);
+    }
+    cp_async_commit();
+  };
+  load_block(0);
+
+  // this warp's 16 query rows, rounded once, in its own slice of shared memory (rows >= N repeat row N - 1 and are
+  // never stored); the fragments are reloaded per key block rather than held in 32 registers
+  const int q0 = blockIdx.x * kTfRows + warp * 16;
+  const bool active = q0 < N;
+  float* sQ = tsm + 2 * kTfStageFloats + warp * 16 * kTfLdK;
+  for (int idx = lane; idx < 16 * (kDH / 4); idx += 32) {
+    const int r = idx >> 4, c = idx & 15;
+    const float4 x = __ldg(reinterpret_cast<const float4*>(base + (long)min(q0 + r, N - 1) * ld + c * 4));
+    *reinterpret_cast<uint4*>(sQ + r * kTfLdK + c * 4) =
+        make_uint4(tf32_rna(x.x), tf32_rna(x.y), tf32_rna(x.z), tf32_rna(x.w));
+  }
+  __syncwarp();
+  float o[kDH / 8][4];
+#pragma unroll
+  for (int i = 0; i < kDH / 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY};
+  float l_run[2] = {0.f, 0.f};
+
+#pragma unroll 1
+  for (int kb = 0; kb < nblocks; ++kb) {
+    if (kb + 1 < nblocks) {
+      load_block(kb + 1);   // its stage was released by the __syncthreads that ended block kb - 1
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    __syncthreads();
+    if (active) {
+      const float* sK = tsm + (kb & 1) * kTfStageFloats;
+      const float* sV = sK + kTfKeys * kTfLdK;
+      const int key0 = kb * kTfKeys;
+      float s[8][4];
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt) s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
+#pragma unroll
+      for (int ks = 0; ks < kDH / 8; ++ks) {
+        const float2 qa = *reinterpret_cast<const float2*>(sQ + g * kTfLdK + 8 * ks + 2 * t);
+        const float2 qb = *reinterpret_cast<const float2*>(sQ + (g + 8) * kTfLdK + 8 * ks + 2 * t);
+        const uint32_t a[4] = {__float_as_uint(qa.x), __float_as_uint(qb.x), __float_as_uint(qa.y), __float_as_uint(qb.y)};
+#pragma unroll
+        for (int nt = 0; nt < 8; ++nt) {
+          const float2 kv = *reinterpret_cast<const float2*>(sK + (nt * 8 + g) * kTfLdK + 8 * ks + 2 * t);
+          mma_tf32_1688(s[nt], a, tf32_rna(kv.x), tf32_rna(kv.y));
+        }
+      }
+      // scale, mask, row max (accumulator element e: row g + 8 (e / 2), key 8 nt + 2t + e % 2)
+      float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int key = key0 + nt * 8 + 2 * t + (e & 1);
+          const float val = key < N ? s[nt][e] * scale_log2 : -INFINITY;
+          s[nt][e] = val;
+          mx[e >> 1] = fmaxf(mx[e >> 1], val);
+        }
+      }
+      float alpha[2];
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+        const float m_new = fmaxf(m_run[r], mx[r]);
+        alpha[r] = exp2f(m_run[r] - m_new);
+        m_run[r] = m_new;
+        l_run[r] *= alpha[r];
+      }
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float pv = exp2f(s[nt][e] - m_run[e >> 1]);
+          s[nt][e] = pv;
+          l_run[e >> 1] += pv;   // the row sum of the unrounded fp32 P
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < kDH / 8; ++i) {
+        o[i][0] *= alpha[0]; o[i][1] *= alpha[0];
+        o[i][2] *= alpha[1]; o[i][3] *= alpha[1];
+      }
+      // O += P V
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt) {
+        const uint32_t a[4] = {tf32_rna(s[nt][0]), tf32_rna(s[nt][2]), tf32_rna(s[nt][1]), tf32_rna(s[nt][3])};
+        const float* v0 = sV + (nt * 8 + 2 * t) * kTfLdV + g;
+#pragma unroll
+        for (int jd = 0; jd < kDH / 8; ++jd)
+          mma_tf32_1688(o[jd], a, tf32_rna(v0[8 * jd]), tf32_rna(v0[kTfLdV + 8 * jd]));
+      }
+    }
+    __syncthreads();   // every warp is done with this stage before block kb + 2 is loaded into it
+  }
+
+  if (!active) return;
+  float inv[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    float l = l_run[r];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    inv[r] = 1.0f / l;
+  }
+  const long ldo = (long)H * kDH;
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int row = q0 + g + 8 * hr;
+    if (row < N) {
+      float* dst = out + ((long)b * N + row) * ldo + h * kDH + 2 * t;
+#pragma unroll
+      for (int jd = 0; jd < kDH / 8; ++jd)
+        *reinterpret_cast<float2*>(dst + 8 * jd) = make_float2(o[jd][2 * hr] * inv[hr], o[jd][2 * hr + 1] * inv[hr]);
+    }
+  }
+}
+
 // ---- fp32 reference-precision path: one warp per (b, h, query) ----
 // Also serves Swin windows: optional additive bias[h, n, n] and mask[w % nmask, n, n]
 // (tfimm/architectures/swin.py:172-194), where "b" enumerates windows.
@@ -283,6 +448,25 @@ int attention_bf16(const void* qkv, void* out, int B, int N, int H, int dh, floa
   // (vit_base_patch8_224 has N = 785); longer sequences are kUnsupported (the host falls back to the fp32 kernel)
   if (N <= 128 || N > 784) return launch_vit_attention<4, 2>(q, o, B, N, H, scale, stream);
   return launch_vit_attention<7, 2>(q, o, B, N, H, scale, stream);
+}
+
+int attention_tf32(const float* qkv, float* out, int B, int N, int H, int dh, float scale, cudaStream_t stream) {
+  TFIMM_CHECK_ARG(B > 0 && N > 0 && H > 0, "attention_tf32: bad shape B=%d N=%d H=%d", B, N, H);
+  if (dh != kDH) {
+    set_last_error("attention_tf32: head_dim 64 only (got %d)", dh);
+    return kUnsupported;
+  }
+  TFIMM_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15u) == 0 && (reinterpret_cast<uintptr_t>(out) & 15u) == 0,
+                  "attention_tf32: pointers must be 16-byte aligned");
+  static unsigned long long attr_devs = 0;
+  if (first_use_on_device(attr_devs))
+    TFIMM_CUDA_OK(cudaFuncSetAttribute(vit_attention_tf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)kTfSmemBytes));
+  dim3 grid((N + kTfRows - 1) / kTfRows, H, B);
+  vit_attention_tf32_kernel<<<grid, kTfWarps * 32, kTfSmemBytes, stream>>>(qkv, out, N, H,
+                                                                           scale * 1.4426950408889634f);
+  TFIMM_LAUNCH_OK("vit_attention_tf32_kernel");
+  return kOk;
 }
 
 int attention_f32(const float* qkv, float* out, const float* bias, const float* mask, int nmask, long B,

@@ -524,6 +524,25 @@ __device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
+// ---- TF32 (precision="tf32") ----
+// fp32 -> TF32 (10 explicit mantissa bits, low 13 bits of the result zero): round to nearest, ties away from zero.
+// Finite values at the top of the range round up to +-inf; NaN and inf pass through.  Every TF32 operand is rounded by
+// this instruction (the tensor core would otherwise use the low bits as it pleases), and the plan-time weight rounding
+// (tfimm.backend.lib.round_tf32) is the same function.
+__device__ __forceinline__ uint32_t tf32_rna(float x) {
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+  return r;
+}
+// D(16x8, f32) += A(16x8, tf32, row) * B(8x8, tf32, col)
+__device__ __forceinline__ void mma_tf32_1688(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 "
+      "{%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
 #endif  // __CUDACC__
 
 }  // namespace tfimm

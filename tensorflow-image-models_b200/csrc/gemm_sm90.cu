@@ -14,7 +14,14 @@
 //               fp32 accumulators in registers, one wgmma group kept in flight (the stage of the group before it is
 //               released as soon as it retires); then the epilogue straight from the fragments (gemm_epilogue.cuh)
 //   warp 8      TMA producer: A/W tiles -> 128B-swizzled smem ring (mbarrier full/empty)
-//   warps 9..12 (gated instances only) squeeze-excite gate applied to the A tile in smem before the MMA reads it
+//   warps 9..12 (A-transform instances only) rewrite the A tile in smem before the MMA reads it: the squeeze-excite
+//               gate (bf16), or the TF32 rounding of fp32 activations (precision="tf32")
+//
+// Operands: bf16 (wgmma k16), or fp32 rounded to TF32 (wgmma k8).  Either way a tile row is 128 bytes -- one
+// SWIZZLE_128B span of 64 bf16 or 32 fp32 contraction indices -- so stage bytes, descriptors and the 32-byte k-step are
+// the same; only the TMA element type, the k-block width and the MMA instruction differ.
+#include <type_traits>
+
 #include "gemm_epilogue.cuh"
 #include "wgmma.cuh"
 
@@ -23,30 +30,44 @@ namespace tfimm {
 namespace {
 
 constexpr int kBlockM = 128;
-constexpr int kBlockK = 64;   // 64 bf16 = one 128-byte swizzle span
+constexpr int kRowBytes = 128;   // one 128-byte swizzle span per tile row
 constexpr int kConsumerThreads = 256;
 constexpr int kProducerWarp = kConsumerThreads / 32;
-constexpr int kNumGateWarps = 4;   // gated instances only: one thread per A-tile row
+constexpr int kNumGateWarps = 4;   // A-transform instances only
+
+// What the A-transform warps do to each A tile between the TMA load and the MMA.
+enum ATransform : int {
+  kANone = 0,   // nothing: the consumers wait on the TMA barrier directly
+  kAGate = 1,   // bf16 A: x * gate[image][k] in fp32, rounded back to bf16 (squeeze-excite)
+  kATf32 = 2,   // fp32 A: cvt.rna.tf32 of every element (precision="tf32")
+};
+template <int AX>
+using OperandT = std::conditional_t<AX == kATf32, float, __nv_bfloat16>;
+template <int AX>
+constexpr int block_k() { return kRowBytes / (int)sizeof(OperandT<AX>); }   // 64 bf16 / 32 fp32
+template <int AX>
+constexpr int dtype_code() { return AX == kATf32 ? kF32 : kBF16; }
 
 template <int BLOCK_N>
 struct GemmCfg {
-  static constexpr int kABytes = kBlockM * kBlockK * 2;
-  static constexpr int kBBytes = BLOCK_N * kBlockK * 2;
+  static constexpr int kABytes = kBlockM * kRowBytes;
+  static constexpr int kBBytes = BLOCK_N * kRowBytes;
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kStages = 4;   // 192 / 128 / 96 KB: BLOCK_N = 64 leaves room for two CTAs per SM
-  static constexpr int kNumBarriers = 3 * kStages;   // full, empty, ready (gated)
+  static constexpr int kNumBarriers = 3 * kStages;   // full, empty, ready (A-transform instances)
   static constexpr int kSmemBytes = kStages * kStageBytes + kNumBarriers * 8 + 1024 /*alignment slack*/;
 };
 
-template <int BLOCK_N, bool kGated>
-constexpr int gemm_threads() { return kConsumerThreads + 32 + (kGated ? 32 * kNumGateWarps : 0); }
+template <int BLOCK_N, int AX>
+constexpr int gemm_threads() { return kConsumerThreads + 32 + (AX != kANone ? 32 * kNumGateWarps : 0); }
 
-template <int BLOCK_N, typename OutT, bool kGated = false>
-__global__ void __launch_bounds__(gemm_threads<BLOCK_N, kGated>(), (BLOCK_N == 64 && !kGated) ? 2 : 1)
-gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+template <int BLOCK_N, typename OutT, int AX = kANone>
+__global__ void __launch_bounds__(gemm_threads<BLOCK_N, AX>(), (BLOCK_N == 64 && AX == kANone) ? 2 : 1)
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                        const GemmParams p) {
   using Cfg = GemmCfg<BLOCK_N>;
   constexpr int kStages = Cfg::kStages;
+  constexpr int kBlockK = block_k<AX>();
 
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles need 1024-byte alignment.
@@ -89,7 +110,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
         if (p.conv == 0) {
           tma_load_2d(sa, &tmap_a, full_bar(stage), kb * kBlockK, m_blk * kBlockM);
         } else {
-          // implicit convolution: tap (ky, kx) and a 64-channel slice of the input patch; padding = OOB zero fill
+          // implicit convolution: tap (ky, kx) and a kBlockK-channel slice of the input patch; padding = OOB zero fill
           const int tap = kb / p.cv_cblocks, cb = kb - tap * p.cv_cblocks;
           const int ky = tap / p.cv_ks, kx = tap - ky * p.cv_ks;
           const int tx = m_blk % p.cv_tiles_x, tyb = m_blk / p.cv_tiles_x;
@@ -101,14 +122,16 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
         if (++stage == kStages) { stage = 0; phase ^= 1u; }
       }
     }
-  } else if (kGated && warp_idx > kProducerWarp) {
-    // ------------------------- A-operand gate (squeeze-excite) -------------------------
-    // Each of the four warps owns every fourth k-block (a whole 128 x 64 tile), so four stages are being rescaled at
-    // any time.  lane = one 16-byte chunk column (8 contraction indices) x 32 rows 4 apart: the gate values of a lane
-    // change only when its rows cross into the next image; a quarter-warp touches one whole 128-byte row (no bank
-    // conflicts under the 128B swizzle).  x * gate in fp32, back as bf16 -- the rounding of the separate scale pass
-    // (csrc/conv.cu, scale_channels_kernel) -- then the proxy fence that makes the generic-proxy writes visible to the
-    // tensor core's async-proxy reads, and one arrive on the stage's "ready" barrier.
+  } else if (AX != kANone && warp_idx > kProducerWarp) {
+    // ------------------------------ A-tile transform ------------------------------
+    // Each of the four warps owns every fourth k-block (a whole 128-row tile), so four stages are being rewritten at
+    // any time.  lane = one 16-byte chunk column x 32 rows 4 apart; a quarter-warp touches one whole 128-byte row (no
+    // bank conflicts under the 128B swizzle).  After the rewrite: the proxy fence that makes the generic-proxy writes
+    // visible to the tensor core's async-proxy reads, and one arrive on the stage's "ready" barrier.
+    //   kAGate: x * gate in fp32, back as bf16 -- the rounding of the separate scale pass (csrc/conv.cu,
+    //           scale_channels_kernel).  A chunk is 8 contraction indices; the gate values of a lane change only when
+    //           its rows cross into the next image.
+    //   kATf32: every element rounded to TF32 (cvt.rna), in place: elementwise, so the swizzle does not matter.
     const int wt = warp_idx - kProducerWarp - 1;
     const int c = lane & 7, r0 = lane >> 3;
     auto load_gate = [&](int img, int k0, float4& ga, float4& gb) {
@@ -116,24 +139,22 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
       ga = __ldg(reinterpret_cast<const float4*>(g));
       gb = __ldg(reinterpret_cast<const float4*>(g + 4));
     };
-    const long row_first = (long)m_blk * kBlockM + r0;
-    long im0 = row_first / p.a_rows_per_img;
-    im0 = im0 < p.a_imgs ? im0 : p.a_imgs - 1;            // rows past M are zero-filled: any gate row will do
-    const int img0 = (int)im0;
-    const long bound0 = (im0 + 1) * p.a_rows_per_img - (long)m_blk * kBlockM;   // first tile row of the next image
+    int img0 = 0;
+    long bound0 = 0;
+    if constexpr (AX == kAGate) {
+      const long row_first = (long)m_blk * kBlockM + r0;
+      long im0 = row_first / p.a_rows_per_img;
+      im0 = im0 < p.a_imgs ? im0 : p.a_imgs - 1;            // rows past M are zero-filled: any gate row will do
+      img0 = (int)im0;
+      bound0 = (im0 + 1) * p.a_rows_per_img - (long)m_blk * kBlockM;   // first tile row of the next image
+    }
     int stage = 0, turn = 0;   // stage / owner of the NEXT k-block
     uint32_t phase = 0;
     for (int kb = 0; kb < num_k_blocks; ++kb) {
       if (turn == wt) {
-        const int k0 = kb * kBlockK + c * 8;
-        const bool valid = k0 < p.K;                       // K % 8 == 0: a chunk is inside or outside as a whole
-        float4 ga = make_float4(0.f, 0.f, 0.f, 0.f), gb = ga;
-        if (valid) load_gate(img0, k0, ga, gb);
-        mbar_wait(full_bar(stage), phase);
-        if (valid) {
+        if constexpr (AX == kATf32) {
+          mbar_wait(full_bar(stage), phase);
           const uint32_t sa = smem_tiles + stage * Cfg::kStageBytes;
-          int cur = img0;
-          long bound = bound0;
 #pragma unroll 1
           for (int b8 = 0; b8 < 4; ++b8) {
             uint4 u[8];
@@ -142,22 +163,52 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
               const int r = r0 + 4 * (8 * b8 + i);
               asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];"
                            : "=r"(u[i].x), "=r"(u[i].y), "=r"(u[i].z), "=r"(u[i].w)
-                           : "r"(sa + (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4))));
+                           : "r"(sa + (uint32_t)(r * 128 + (c << 4))));
             }
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
               const int r = r0 + 4 * (8 * b8 + i);
-              if (r >= bound && cur < p.a_imgs - 1) {
-                do { ++cur; bound += p.a_rows_per_img; } while (r >= bound && cur < p.a_imgs - 1);
-                load_gate(cur, k0, ga, gb);
-              }
-              const float2 x0 = unpack_bf16x2(u[i].x), x1 = unpack_bf16x2(u[i].y), x2 = unpack_bf16x2(u[i].z),
-                           x3 = unpack_bf16x2(u[i].w);
-              const uint32_t o0 = pack_bf16x2(x0.x * ga.x, x0.y * ga.y), o1 = pack_bf16x2(x1.x * ga.z, x1.y * ga.w);
-              const uint32_t o2 = pack_bf16x2(x2.x * gb.x, x2.y * gb.y), o3 = pack_bf16x2(x3.x * gb.z, x3.y * gb.w);
-              asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(sa + (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4))),
-                           "r"(o0), "r"(o1), "r"(o2), "r"(o3)
+              asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(sa + (uint32_t)(r * 128 + (c << 4))),
+                           "r"(tf32_rna(__uint_as_float(u[i].x))), "r"(tf32_rna(__uint_as_float(u[i].y))),
+                           "r"(tf32_rna(__uint_as_float(u[i].z))), "r"(tf32_rna(__uint_as_float(u[i].w)))
                            : "memory");
+            }
+          }
+        } else {
+          const int k0 = kb * kBlockK + c * 8;
+          const bool valid = k0 < p.K;                       // K % 8 == 0: a chunk is inside or outside as a whole
+          float4 ga = make_float4(0.f, 0.f, 0.f, 0.f), gb = ga;
+          if (valid) load_gate(img0, k0, ga, gb);
+          mbar_wait(full_bar(stage), phase);
+          if (valid) {
+            const uint32_t sa = smem_tiles + stage * Cfg::kStageBytes;
+            int cur = img0;
+            long bound = bound0;
+#pragma unroll 1
+            for (int b8 = 0; b8 < 4; ++b8) {
+              uint4 u[8];
+#pragma unroll
+              for (int i = 0; i < 8; ++i) {
+                const int r = r0 + 4 * (8 * b8 + i);
+                asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];"
+                             : "=r"(u[i].x), "=r"(u[i].y), "=r"(u[i].z), "=r"(u[i].w)
+                             : "r"(sa + (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4))));
+              }
+#pragma unroll
+              for (int i = 0; i < 8; ++i) {
+                const int r = r0 + 4 * (8 * b8 + i);
+                if (r >= bound && cur < p.a_imgs - 1) {
+                  do { ++cur; bound += p.a_rows_per_img; } while (r >= bound && cur < p.a_imgs - 1);
+                  load_gate(cur, k0, ga, gb);
+                }
+                const float2 x0 = unpack_bf16x2(u[i].x), x1 = unpack_bf16x2(u[i].y), x2 = unpack_bf16x2(u[i].z),
+                             x3 = unpack_bf16x2(u[i].w);
+                const uint32_t o0 = pack_bf16x2(x0.x * ga.x, x0.y * ga.y), o1 = pack_bf16x2(x1.x * ga.z, x1.y * ga.w);
+                const uint32_t o2 = pack_bf16x2(x2.x * gb.x, x2.y * gb.y), o3 = pack_bf16x2(x3.x * gb.z, x3.y * gb.w);
+                asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};"
+                             ::"r"(sa + (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4))), "r"(o0), "r"(o1), "r"(o2), "r"(o3)
+                             : "memory");
+              }
             }
           }
         }
@@ -178,14 +229,20 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     int stage = 0, prev = 0;
     uint32_t phase = 0;
     for (int kb = 0; kb < num_k_blocks; ++kb) {
-      mbar_wait(kGated ? ready_bar(stage) : full_bar(stage), phase);   // gated: the A tile has been rescaled
+      // A-transform instances: the A tile has been rewritten
+      mbar_wait(AX != kANone ? ready_bar(stage) : full_bar(stage), phase);
       const uint32_t sa = smem_tiles + stage * Cfg::kStageBytes;
       const uint64_t da = gmma_desc_k_sw128(sa + (uint32_t)wg * (64 * 128));
       const uint64_t db = gmma_desc_k_sw128(sa + Cfg::kABytes);
       wgmma_fence();
+      // four 32-byte k-steps per 128-byte row (k16 bf16 / k8 tf32): +2 on the descriptors each
 #pragma unroll
-      for (int k = 0; k < kBlockK / 16; ++k)
-        wgmma_ss<BLOCK_N>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (uint32_t)((kb | k) != 0));
+      for (int k = 0; k < 4; ++k) {
+        if constexpr (AX == kATf32)
+          wgmma_ss_tf32<BLOCK_N>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (uint32_t)((kb | k) != 0));
+        else
+          wgmma_ss<BLOCK_N>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (uint32_t)((kb | k) != 0));
+      }
       wgmma_commit();
       // the group issued one k-block ago has retired: its stage may be refilled
       wgmma_wait<1>();
@@ -209,25 +266,26 @@ int check_out(const void* C, long ldc, const void* residual, long ldr, int esize
   return kOk;
 }
 
-template <int BLOCK_N, typename OutT, bool kGated = false>
+template <int BLOCK_N, typename OutT, int AX = kANone>
 int launch_gemm(const void* A, int lda, const void* W, int ldw, const void* residual, int ldr, void* C, int ldc,
                 GemmParams p, cudaStream_t stream) {
   const int M = p.M, N = p.N, K = p.K;
   using Cfg = GemmCfg<BLOCK_N>;
+  constexpr int kBlockK = block_k<AX>();
   CUtensorMap ta, tb;
   int st;
   if ((st = check_out(C, ldc, residual, ldr, (int)sizeof(OutT))) != kOk) return st;
-  if ((st = make_tmap_2d(&ta, A, kBF16, M, K, lda, kBlockM, kBlockK, "A")) != kOk) return st;
-  if ((st = make_tmap_2d(&tb, W, kBF16, N, K, ldw, BLOCK_N, kBlockK, "W")) != kOk) return st;
+  if ((st = make_tmap_2d(&ta, A, dtype_code<AX>(), M, K, lda, kBlockM, kBlockK, "A")) != kOk) return st;
+  if ((st = make_tmap_2d(&tb, W, dtype_code<AX>(), N, K, ldw, BLOCK_N, kBlockK, "W")) != kOk) return st;
   p.c = C; p.res = residual; p.ldc = ldc; p.ldr = ldr;
-  auto kernel = gemm_bf16_wgmma_kernel<BLOCK_N, OutT, kGated>;
+  auto kernel = gemm_wgmma_kernel<BLOCK_N, OutT, AX>;
   static unsigned long long attr_devs = 0;  // per instantiation
   if (first_use_on_device(attr_devs)) {
     TFIMM_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
   }
   const long tiles = (long)((M + kBlockM - 1) / kBlockM) * ((N + BLOCK_N - 1) / BLOCK_N);
-  kernel<<<(unsigned)tiles, gemm_threads<BLOCK_N, kGated>(), Cfg::kSmemBytes, stream>>>(ta, tb, p);
-  TFIMM_LAUNCH_OK("gemm_bf16_wgmma_kernel");
+  kernel<<<(unsigned)tiles, gemm_threads<BLOCK_N, AX>(), Cfg::kSmemBytes, stream>>>(ta, tb, p);
+  TFIMM_LAUNCH_OK(AX == kATf32 ? "gemm_wgmma_kernel (tf32)" : "gemm_wgmma_kernel (bf16)");
   return kOk;
 }
 
@@ -235,32 +293,35 @@ int pick_block_n(int M, int N);
 
 // Implicit k x k convolution on the tensor cores: same kernel, A tensor map = the NHWC input (rank 4, traversal
 // stride = conv stride), C / residual = the NHWC output.  See GemmParams::conv.
-template <int BLOCK_N, typename OutT>
+template <int BLOCK_N, typename OutT, int AX = kANone>
 int launch_conv(const void* x, const void* W, int ldw, const void* residual, void* out, int B, int H, int Wd, int C,
                 int Ho, int Wo, GemmParams p, cudaStream_t stream) {
   using Cfg = GemmCfg<BLOCK_N>;
+  constexpr int kBlockK = block_k<AX>();
+  constexpr uint64_t es = sizeof(OperandT<AX>);
   const int N = p.N, s = p.cv_stride;
   CUtensorMap ta, tb;
   int st;
   if ((st = check_out(out, N, residual, N, (int)sizeof(OutT))) != kOk) return st;
   {
     const uint64_t dims[4] = {(uint64_t)C, (uint64_t)Wd, (uint64_t)H, (uint64_t)B};
-    const uint64_t strides[3] = {(uint64_t)C * 2, (uint64_t)Wd * C * 2, (uint64_t)H * Wd * C * 2};
+    const uint64_t strides[3] = {(uint64_t)C * es, (uint64_t)Wd * C * es, (uint64_t)H * Wd * C * es};
     const uint32_t box[4] = {(uint32_t)kBlockK, (uint32_t)(p.cv_pw * s), (uint32_t)(p.cv_ph * s), (uint32_t)p.cv_pb};
     const uint32_t estr[4] = {1u, (uint32_t)s, (uint32_t)s, 1u};
-    if ((st = make_tmap(&ta, x, kBF16, 4, dims, strides, box, "conv input", 128, estr)) != kOk) return st;
+    if ((st = make_tmap(&ta, x, dtype_code<AX>(), 4, dims, strides, box, "conv input", 128, estr)) != kOk) return st;
   }
-  if ((st = make_tmap_2d(&tb, W, kBF16, N, p.K, ldw, BLOCK_N, kBlockK, "conv weights")) != kOk) return st;
+  if ((st = make_tmap_2d(&tb, W, dtype_code<AX>(), N, p.K, ldw, BLOCK_N, kBlockK, "conv weights")) != kOk) return st;
   p.c = out; p.res = residual; p.ldc = N; p.ldr = N;
   p.cv_B = B; p.cv_Ho = Ho; p.cv_Wo = Wo;
-  auto kernel = gemm_bf16_wgmma_kernel<BLOCK_N, OutT>;
+  auto kernel = gemm_wgmma_kernel<BLOCK_N, OutT, AX>;
   static unsigned long long attr_devs = 0;  // per instantiation
   if (first_use_on_device(attr_devs)) {
     TFIMM_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
   }
   const long tiles = (long)(p.M / kBlockM) * ((N + BLOCK_N - 1) / BLOCK_N);
-  kernel<<<(unsigned)tiles, gemm_threads<BLOCK_N, false>(), Cfg::kSmemBytes, stream>>>(ta, tb, p);
-  TFIMM_LAUNCH_OK("gemm_bf16_wgmma_kernel (implicit convolution)");
+  kernel<<<(unsigned)tiles, gemm_threads<BLOCK_N, AX>(), Cfg::kSmemBytes, stream>>>(ta, tb, p);
+  TFIMM_LAUNCH_OK(AX == kATf32 ? "gemm_wgmma_kernel (tf32 implicit convolution)"
+                                  : "gemm_wgmma_kernel (bf16 implicit convolution)");
   return kOk;
 }
 
@@ -343,27 +404,28 @@ int gemm_bf16_gated_dispatch(const void* A, int lda, const float* gate, int rows
   // at most 128 columns: the gate warps leave the consumers too few registers for a 256-wide accumulator
   switch (pick_block_n(M, N)) {
     case 256:
-    case 128: return launch_gemm<128, __nv_bfloat16, true>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream);
-    default: return launch_gemm<64, __nv_bfloat16, true>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream);
+    case 128: return launch_gemm<128, __nv_bfloat16, kAGate>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream);
+    default: return launch_gemm<64, __nv_bfloat16, kAGate>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream);
   }
 }
 
 // k x k convolution (stride 1 or 2, symmetric padding (k-1)/2... given as `pad`) + bias + activation (+ residual),
 // NHWC bf16 in, NHWC bf16/fp32 out, W[N][k*k*C] in (ky, kx, c) order: implicit GEMM, no im2col matrix in HBM.
-int conv_bf16_dispatch(const void* x, const void* W, int ldw, const float* bias, const void* residual, void* out,
-                       int B, int H, int Wd, int C, int N, int ks, int stride, int pad, int act, int act_post,
-                       int out_dtype, cudaStream_t stream) {
-  TFIMM_CHECK_ARG(B > 0 && H > 0 && Wd > 0 && C > 0 && C % 64 == 0, "conv: C must be a multiple of 64 (got %d)", C);
+// Geometry of an implicit convolution (shared by the bf16 and TF32 entry points); `cblock` = channels per k-block.
+int conv_setup(GemmParams& p, const float* bias, const void* residual, int B, int H, int Wd, int C, int N, int ks,
+               int stride, int pad, int act, int act_post, int cblock, int& Ho, int& Wo) {
+  TFIMM_CHECK_ARG(B > 0 && H > 0 && Wd > 0 && C > 0 && C % cblock == 0, "conv: C must be a multiple of %d (got %d)",
+                  cblock, C);
   TFIMM_CHECK_ARG(ks >= 1 && ks <= 7 && (stride == 1 || stride == 2) && pad >= 0 && pad < ks, "conv: bad geometry");
   TFIMM_CHECK_ARG(N > 0 && N % 8 == 0, "conv: N must be a multiple of 8 (got %d)", N);
-  TFIMM_CHECK_ARG(out_dtype == kBF16 || out_dtype == kF32, "conv: out_dtype must be bf16 or f32");
   TFIMM_CHECK_ARG(bias == nullptr || (reinterpret_cast<uintptr_t>(bias) & 15u) == 0, "conv: bias must be 16-byte aligned");
-  const int Ho = (H + 2 * pad - ks) / stride + 1, Wo = (Wd + 2 * pad - ks) / stride + 1;
+  Ho = (H + 2 * pad - ks) / stride + 1;
+  Wo = (Wd + 2 * pad - ks) / stride + 1;
   TFIMM_CHECK_ARG(Ho > 0 && Wo > 0, "conv: empty output");
-  GemmParams p{};
+  p = GemmParams{};
   p.N = N; p.K = ks * ks * C;
   p.bias = bias; p.act = act; p.has_res = residual != nullptr ? 1 : 0; p.act_post = act_post;
-  p.conv = 1; p.cv_cblocks = C / 64; p.cv_ks = ks; p.cv_stride = stride; p.cv_pad = pad;
+  p.conv = 1; p.cv_cblocks = C / cblock; p.cv_ks = ks; p.cv_stride = stride; p.cv_pad = pad;
   // 128-pixel output patch: 8 x 16 pixels of one image, or 8 x 8 pixels of two images for small feature maps
   if (Wo > 8) { p.cv_pb = 1; p.cv_ph = 8; p.cv_pw = 16; }
   else { p.cv_pb = 2; p.cv_ph = 8; p.cv_pw = 8; }
@@ -371,6 +433,17 @@ int conv_bf16_dispatch(const void* x, const void* W, int ldw, const float* bias,
   p.cv_tiles_y = (Ho + p.cv_ph - 1) / p.cv_ph;
   const int tiles_b = (B + p.cv_pb - 1) / p.cv_pb;
   p.M = tiles_b * p.cv_tiles_y * p.cv_tiles_x * kBlockM;  // padded row count: every tile is a full patch
+  return kOk;
+}
+
+int conv_bf16_dispatch(const void* x, const void* W, int ldw, const float* bias, const void* residual, void* out,
+                       int B, int H, int Wd, int C, int N, int ks, int stride, int pad, int act, int act_post,
+                       int out_dtype, cudaStream_t stream) {
+  TFIMM_CHECK_ARG(out_dtype == kBF16 || out_dtype == kF32, "conv: out_dtype must be bf16 or f32");
+  GemmParams p;
+  int Ho, Wo, st;
+  if ((st = conv_setup(p, bias, residual, B, H, Wd, C, N, ks, stride, pad, act, act_post, 64, Ho, Wo)) != kOk)
+    return st;
   const int bn = N >= 256 ? 256 : (N >= 128 ? 128 : 64);
 #define TFIMM_CONV_CASE(BN)                                                                                       \
   case BN:                                                                                                        \
@@ -384,6 +457,45 @@ int conv_bf16_dispatch(const void* x, const void* W, int ldw, const float* bias,
   }
 #undef TFIMM_CONV_CASE
   return kInvalidArgument;
+}
+
+// ---- precision="tf32": fp32 operands, TF32 tensor-core products, fp32 out ----
+// W must already be TF32-representable (low 13 bits zero: rounded once at plan time); the A tiles are rounded in shared
+// memory by the transform warps.  At most 128 columns: the transform warps leave the consumers too few registers for a
+// 256-wide accumulator (as in the gated instances).
+int gemm_tf32_dispatch(const float* A, int lda, const float* W, int ldw, const float* bias, const float* gamma,
+                       const float* residual, int ldr, float* C, int ldc, int M, int N, int K, int act, int act_post,
+                       int force_block_n, cudaStream_t stream) {
+  TFIMM_CHECK_ARG(M > 0 && N > 0 && K > 0, "gemm_tf32: M, N, K must be positive (got %d %d %d)", M, N, K);
+  TFIMM_CHECK_ARG(K % 4 == 0, "gemm_tf32: K must be a multiple of 4 (got %d)", K);
+  TFIMM_CHECK_ARG(bias == nullptr || (reinterpret_cast<uintptr_t>(bias) & 15u) == 0, "gemm_tf32: bias must be 16-byte aligned");
+  TFIMM_CHECK_ARG(gamma == nullptr || (reinterpret_cast<uintptr_t>(gamma) & 15u) == 0,
+                  "gemm_tf32: gamma must be 16-byte aligned");
+  GemmParams p{};
+  p.M = M; p.N = N; p.K = K;
+  p.bias = bias; p.gamma = gamma; p.act = act; p.has_res = residual != nullptr ? 1 : 0; p.act_post = act_post;
+  // force_block_n: 0 = choose; 64 / 128 = that tile width; 2 = the widest tile (128)
+  const int bn = force_block_n == 2 ? 128 : (force_block_n > 0 ? force_block_n : (pick_block_n(M, N) == 64 ? 64 : 128));
+  switch (bn) {
+    case 128: return launch_gemm<128, float, kATf32>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream);
+    case 64: return launch_gemm<64, float, kATf32>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream);
+    default:
+      set_last_error("gemm_tf32: unsupported block_n %d (64 or 128)", bn);
+      return kInvalidArgument;
+  }
+}
+
+// k x k convolution as conv_bf16_dispatch, fp32 NHWC in / out with TF32 products; C % 32 == 0 (one 32-channel fp32 box
+// per k-block).
+int conv_tf32_dispatch(const float* x, const float* W, int ldw, const float* bias, const float* residual, float* out,
+                       int B, int H, int Wd, int C, int N, int ks, int stride, int pad, int act, int act_post,
+                       cudaStream_t stream) {
+  GemmParams p;
+  int Ho, Wo, st;
+  if ((st = conv_setup(p, bias, residual, B, H, Wd, C, N, ks, stride, pad, act, act_post, 32, Ho, Wo)) != kOk)
+    return st;
+  if (N >= 128) return launch_conv<128, float, kATf32>(x, W, ldw, residual, out, B, H, Wd, C, Ho, Wo, p, stream);
+  return launch_conv<64, float, kATf32>(x, W, ldw, residual, out, B, H, Wd, C, Ho, Wo, p, stream);
 }
 
 }  // namespace tfimm

@@ -99,6 +99,34 @@ __device__ __forceinline__ void wgmma_rs<256>(float (&d)[128], const uint32_t (&
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
 }
 
+// TF32 form (precision="tf32"): wgmma m64nNk8.f32.tf32.tf32, both operands K-major from shared memory (TF32 takes no
+// transpose immediates).  A k8 step is 32 bytes of a 128-byte swizzle span, like the bf16 k16 step: the descriptors
+// advance identically.
+template <int N>
+__device__ __forceinline__ void wgmma_ss_tf32(float (&d)[N / 2], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate);
+
+template <>
+__device__ __forceinline__ void wgmma_ss_tf32<64>(float (&d)[32], uint64_t a_desc, uint64_t b_desc,
+                                                  uint32_t accumulate) {
+  asm volatile("{.reg .pred p; setp.ne.b32 p, %34, 0; wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,"
+               "%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;}"
+               : TFIMM_F8(0), TFIMM_F8(8), TFIMM_F8(16), TFIMM_F8(24)
+               : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+template <>
+__device__ __forceinline__ void wgmma_ss_tf32<128>(float (&d)[64], uint64_t a_desc, uint64_t b_desc,
+                                                   uint32_t accumulate) {
+  asm volatile("{.reg .pred p; setp.ne.b32 p, %66, 0; wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,"
+               "%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,"
+               "%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,"
+               "%60,%61,%62,%63}, %64, %65, p, 1, 1;}"
+               : TFIMM_F8(0), TFIMM_F8(8), TFIMM_F8(16), TFIMM_F8(24), TFIMM_F8(32), TFIMM_F8(40),
+                 TFIMM_F8(48), TFIMM_F8(56)
+               : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+
 #undef TFIMM_F8
 
 }  // namespace tfimm

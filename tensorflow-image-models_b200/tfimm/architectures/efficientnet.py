@@ -263,7 +263,7 @@ class EfficientNet(Model):
         Kpad = (K + 7) // 8 * 8
         if Kpad != K:
             w2 = torch.nn.functional.pad(w2, (0, Kpad - K))
-        return w2.to(self.act_dtype).contiguous(), shift.contiguous()
+        return self._gemm_operand(w2), shift.contiguous()
 
     def _folded_dw(self, conv_prefix, bn_prefix):
         scale, shift = self._bn_scale_shift(bn_prefix)

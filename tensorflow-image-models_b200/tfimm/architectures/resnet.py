@@ -239,7 +239,7 @@ class ResNet(Model):
         Kpad = (K + 7) // 8 * 8
         if Kpad != K:
             w2 = torch.nn.functional.pad(w2, (0, Kpad - K))
-        return w2.to(self.act_dtype).contiguous(), shift, gn
+        return self._gemm_operand(w2), shift, gn
 
     def _folded_grouped_wide(self, conv_prefix, bn_prefix, groups):
         """Grouped 3x3 with >= 48 channels per group: one [cg][Kpad] GEMM weight per group (see _grouped_wide)."""
@@ -250,7 +250,7 @@ class ResNet(Model):
         Kpad = (k * k * cg + 7) // 8 * 8
         if Kpad != k * k * cg:
             wg = torch.nn.functional.pad(wg, (0, Kpad - k * k * cg))
-        return wg.to(self.act_dtype).contiguous(), shift.contiguous()
+        return self._gemm_operand(wg), shift.contiguous()
 
     def _folded_grouped(self, conv_prefix, bn_prefix):
         scale, shift = self._bn_scale_shift(bn_prefix)
@@ -294,7 +294,7 @@ class ResNet(Model):
     def _conv(self, x, wb, k, stride, pad, act, residual=None, act_after_residual=False):
         w, bias, gn = wb
         B = x.shape[0]
-        if (k > 1 and gn is None and self.precision == "bf16" and isinstance(pad, int) and x.shape[-1] % 64 == 0
+        if (k > 1 and gn is None and self.precision in ("bf16", "tf32") and isinstance(pad, int) and x.shape[-1] % 64 == 0
                 and w.shape[1] == k * k * x.shape[-1]):
             # implicit GEMM: the A tiles are 4-D TMA boxes of the feature map, nothing is materialised
             return ops.conv_gemm(x, w, bias=bias, ks=k, stride=stride, pad=pad, act=act,

@@ -5,6 +5,7 @@ does not need a GPU (cudart is linked statically and the driver entry points are
 lazily), so the CPU test-suite can check that every declared symbol is exported.  There is
 no CPU fallback: if the library is missing, every kernel call raises.
 """
+import contextvars
 import ctypes
 import os
 from pathlib import Path
@@ -30,6 +31,9 @@ SIGNATURES = {
     "tfimm_b200_gemm_bf16": [_P, _I, _P, _I, _P, _P, _P, _I, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P],
     "tfimm_b200_conv_bf16": [_P, _P, _I, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P],
     "tfimm_b200_gemm_f32": [_P, _I, _P, _I, _P, _P, _P, _I, _P, _I, _I, _I, _I, _I, _I, _P],
+    "tfimm_b200_gemm_tf32": [_P, _I, _P, _I, _P, _P, _P, _I, _P, _I, _I, _I, _I, _I, _I, _I, _P],
+    "tfimm_b200_conv_tf32": [_P, _P, _I, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P],
+    "tfimm_b200_attention_tf32": [_P, _P, _I, _I, _I, _I, _F, _P],
     "tfimm_b200_layernorm": [_P, _I, _L, _P, _P, _P, _I, _L, _L, _I, _F, _P],
     "tfimm_b200_layernorm_patch2x2": [_P, _I, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P],
     "tfimm_b200_patch_merge_ln": [_P, _I, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P],
@@ -64,6 +68,27 @@ _SPECIAL = {
 }
 
 _lib = None
+
+# precision="tf32": while set, the fp32 launchers of ``tfimm.backend.ops`` whose contraction has a TF32 tensor-core kernel
+# (gemm, conv_gemm, ViT attention) run it instead of the fp32 SIMT kernel.  A model's public forward entry points
+# (``call``, ``forward_features``: see ``Model.__init_subclass__``) set it to whether the model is a tf32 model and reset
+# it afterwards; a context variable, so threads and asyncio tasks each see their own.
+tf32_mode = contextvars.ContextVar("tfimm_tf32_mode", default=False)
+
+
+def round_tf32(t):
+    """fp32 tensor -> the nearest TF32 value (10 explicit mantissa bits, low 13 bits zero), ties away from zero: what
+    ``cvt.rna.tf32.f32`` computes inside the TF32 kernels.  Finite values at the top of the range round to +-inf;
+    inf and NaN pass through.  Used for GEMM weights, which are rounded once when the plan is built."""
+    import torch
+
+    assert t.dtype == torch.float32, t.dtype
+    bits = t.contiguous().view(torch.int32)
+    finite = (bits & 0x7F800000) != 0x7F800000
+    # adding half a TF32 ulp to the magnitude bits and truncating rounds the magnitude half away from zero; a carry
+    # out of the mantissa correctly bumps the exponent (and the largest binade into inf)
+    rounded = (bits + 0x1000) & ~0x1FFF
+    return torch.where(finite, rounded, bits).view(torch.float32)
 
 
 class KernelLibraryError(RuntimeError):

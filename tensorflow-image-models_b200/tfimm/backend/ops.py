@@ -91,7 +91,7 @@ def act_code(act) -> int:
 def gemm(a, w, bias=None, act=None, gamma=None, residual=None, out=None, out_dtype=None, block_n=0,
          act_after_residual=False):
     """out = residual + gamma * act(a @ w.T + bias)  (act_after_residual: act(residual + gamma*(...))).
-    a:(M,K), w:(N,K); bf16 -> wgmma, fp32 -> SIMT."""
+    a:(M,K), w:(N,K); bf16 -> wgmma, fp32 -> SIMT, or TF32 wgmma in a tf32 model's forward (``lib.tf32_mode``)."""
     _cuda(a, w, bias, gamma, residual, out)
     M, K = a.shape
     N = w.shape[0]
@@ -111,6 +111,13 @@ def gemm(a, w, bias=None, act=None, gamma=None, residual=None, out=None, out_dty
         _call("tfimm_b200_gemm_bf16", a.data_ptr(), a.stride(0), w.data_ptr(), w.stride(0), _ptr(bias),
               _ptr(gamma), _ptr(residual), ldr, out.data_ptr(), out.stride(0), M, N, K, act_code(act),
               int(bool(act_after_residual)), _code(out), block_n, _stream(), flops=2.0 * M * N * K,
+              nbytes=_nbytes(a, w, out, residual))
+    elif _lib.tf32_mode.get():
+        # precision="tf32": w was rounded to TF32 when the plan was built; the kernel rounds the A tiles
+        assert a.dtype == torch.float32 and w.dtype == torch.float32 and out.dtype == torch.float32
+        _call("tfimm_b200_gemm_tf32", a.data_ptr(), a.stride(0), w.data_ptr(), w.stride(0), _ptr(bias),
+              _ptr(gamma), _ptr(residual), ldr, out.data_ptr(), out.stride(0), M, N, K, act_code(act),
+              int(bool(act_after_residual)), block_n, _stream(), flops=2.0 * M * N * K,
               nbytes=_nbytes(a, w, out, residual))
     else:
         assert a.dtype == torch.float32 and w.dtype == torch.float32 and out.dtype == torch.float32
@@ -170,17 +177,26 @@ def mlp_fused(a, w1, b1, w2, b2, act, gamma=None, residual=None, out=None):
 def conv_gemm(x, w, bias=None, ks=3, stride=1, pad=1, act=None, residual=None, act_after_residual=False,
               out_dtype=None):
     """Dense k x k convolution as an implicit GEMM (no im2col matrix).  x: (B,H,W,C) bf16 with C % 64 == 0;
-    w: (N, ks*ks*C) bf16 in (ky, kx, c) order; residual / result: (B,Ho,Wo,N)."""
+    w: (N, ks*ks*C) bf16 in (ky, kx, c) order; residual / result: (B,Ho,Wo,N).  In a tf32 model's forward
+    (``lib.tf32_mode``): x, w, residual and result fp32, C % 32 == 0, TF32 products."""
     _cuda(x, w, bias, residual)
     B, H, W, C = x.shape
     N = w.shape[0]
-    assert x.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and x.is_contiguous() and w.stride(1) == 1
+    tf32 = x.dtype == torch.float32 and _lib.tf32_mode.get()
+    assert x.dtype == w.dtype and (x.dtype == torch.bfloat16 or tf32), (x.dtype, w.dtype)
+    assert x.is_contiguous() and w.stride(1) == 1
     assert w.shape[1] == ks * ks * C, (w.shape, ks, C)
     Ho, Wo = (H + 2 * pad - ks) // stride + 1, (W + 2 * pad - ks) // stride + 1
     out_dtype = out_dtype or (residual.dtype if residual is not None else x.dtype)
     out = torch.empty((B, Ho, Wo, N), device=x.device, dtype=out_dtype)
     if residual is not None:
         assert residual.shape == out.shape and residual.dtype == out.dtype and residual.is_contiguous()
+    if tf32:
+        assert out.dtype == torch.float32
+        _call("tfimm_b200_conv_tf32", x.data_ptr(), w.data_ptr(), w.stride(0), _ptr(bias), _ptr(residual),
+              out.data_ptr(), B, H, W, C, N, ks, stride, pad, act_code(act), int(bool(act_after_residual)), _stream(),
+              flops=2.0 * B * Ho * Wo * N * ks * ks * C, nbytes=_nbytes(x, w, out, residual))
+        return out
     _call("tfimm_b200_conv_bf16", x.data_ptr(), w.data_ptr(), w.stride(0), _ptr(bias), _ptr(residual), out.data_ptr(),
           B, H, W, C, N, ks, stride, pad, act_code(act), int(bool(act_after_residual)), _code(out), _stream(),
           flops=2.0 * B * Ho * Wo * N * ks * ks * C, nbytes=_nbytes(x, w, out, residual))
@@ -234,12 +250,17 @@ def patch_merge_ln(x, gamma, beta, eps, out_dtype):
 
 def attention(qkv, B, N, H, dh, scale, bias=None, mask=None, probs=None, row_map=None, nw_img=0):
     """softmax(scale q k^T [+bias +mask]) v from packed qkv (B*N, 3*H*dh) -> (B*N, H*dh).
-    row_map/nw_img (fp32 only): Swin window permutation folded into addressing."""
+    row_map/nw_img (fp32 only): Swin window permutation folded into addressing.  In a tf32 model's forward, fp32 qkv
+    with head_dim 64 and none of bias / mask / probs / row_map runs the TF32 tensor-core kernel; the rest stays SIMT."""
     _cuda(qkv, bias, mask, probs, row_map)
     assert qkv.shape == (B * N, 3 * H * dh) and qkv.is_contiguous()
     out = torch.empty((B * N, H * dh), device=qkv.device, dtype=qkv.dtype)
-    if qkv.dtype == torch.bfloat16 and bias is None and mask is None and probs is None and row_map is None:
+    plain = bias is None and mask is None and probs is None and row_map is None
+    if qkv.dtype == torch.bfloat16 and plain:
         _call("tfimm_b200_attention_bf16", qkv.data_ptr(), out.data_ptr(), B, N, H, dh, float(scale), _stream(),
+              flops=4.0 * B * H * N * N * dh, nbytes=_nbytes(qkv, out))
+    elif qkv.dtype == torch.float32 and plain and dh == 64 and _lib.tf32_mode.get():
+        _call("tfimm_b200_attention_tf32", qkv.data_ptr(), out.data_ptr(), B, N, H, dh, float(scale), _stream(),
               flops=4.0 * B * H * N * N * dh, nbytes=_nbytes(qkv, out))
     elif qkv.dtype == torch.float32:
         nmask = mask.shape[0] if mask is not None else 1

@@ -10,8 +10,8 @@ Behavioural contract: reference tfimm/models/factory.py:18-305 (see SURVEY.md 8b
   * ``create_preprocessing`` returns ``f(img) = (img / 255 - mean) / std`` with mean / std tiled
     cyclically to ``in_channels``.
 
-Engine-specific keyword arguments (not config fields): ``precision`` ("bf16" default | "fp32"),
-``device`` and ``seed``.  Weight sources available offline: a ``model_path`` / cache entry that is
+Engine-specific keyword arguments (not config fields): ``precision`` ("bf16" default | "fp32" |
+"tf32", see ``tfimm.models.model.PRECISIONS``), ``device`` and ``seed``.  Weight sources available offline: a ``model_path`` / cache entry that is
 a ``.npz`` / ``.pt`` flat dict in reference names, or a PyTorch ``state_dict`` converted by
 ``tfimm.utils.timm`` rules.  Downloading needs a network and raises ``NotImplementedError``.
 """

@@ -12,6 +12,7 @@ Contract kept from the reference (SURVEY.md 8b; e.g. tfimm/architectures/vit.py:
 What is different by design: weights live in HBM as torch CUDA tensors; the forward pass is a
 sequence of hand-written sm_90a kernels (tfimm.backend.ops); inference only.
 """
+import functools
 import math
 from collections import OrderedDict
 from dataclasses import dataclass
@@ -83,10 +84,42 @@ def _init_tensor(spec: ParamSpec, gen: torch.Generator) -> torch.Tensor:
     raise ValueError(f"Unknown initializer {spec.init}")
 
 
+# bf16: bf16 GEMM operands / activations, fp32 accumulation and residual stream (the fast default).
+# fp32: fp32 everywhere on CUDA cores (parity with the reference's arithmetic).
+# tf32: fp32 storage, every contraction (GEMMs, k x k convolutions, ViT self-attention) on the TF32 tensor cores, operands
+#       rounded to TF32 (round to nearest, ties away) -- what TensorFlow runs for fp32 models on Ampere and newer GPUs.
+PRECISIONS = ("bf16", "fp32", "tf32")
+
+
+def _in_precision_mode(forward):
+    """Wraps a public forward entry point (``call``, ``forward_features``): while it runs, the launchers' TF32 switch
+    (``lib.tf32_mode``) is on exactly when the model is a tf32 model -- reset afterwards, also when it raises, and
+    independent of the caller's context."""
+
+    @functools.wraps(forward)
+    def wrapped(self, *args, **kwargs):
+        token = _lib.tf32_mode.set(self.precision == "tf32")
+        try:
+            return forward(self, *args, **kwargs)
+        finally:
+            _lib.tf32_mode.reset(token)
+
+    return wrapped
+
+
 class Model:
     cfg_class = None
     # regexes of weights created at build time that need not be present when loading
     keys_to_ignore_on_load_missing: List[str] = []
+
+    def __init_subclass__(cls, **kwargs):
+        # every public forward entry point of an architecture -- ``model(x)``, ``model.call``,
+        # ``model.forward_features``, and through them ``cuda_graph`` and the serving / parallel paths -- runs its
+        # launches in the model's precision mode
+        super().__init_subclass__(**kwargs)
+        for name in ("call", "forward_features"):
+            if name in cls.__dict__:
+                setattr(cls, name, _in_precision_mode(cls.__dict__[name]))
 
     def __init__(self, cfg, *args, name: Optional[str] = None, precision: str = "bf16",
                  device=None, seed: int = 0, **kwargs):
@@ -94,8 +127,8 @@ class Model:
             cfg = self.cfg_class(**cfg)
         if self.cfg_class is not None and not isinstance(cfg, self.cfg_class):
             raise ValueError("Must pass either `cfg` (ModelConfig) or `cfg` (dict)")
-        if precision not in ("bf16", "fp32"):
-            raise ValueError(f"precision must be 'bf16' or 'fp32', got {precision!r}")
+        if precision not in PRECISIONS:
+            raise ValueError(f"precision must be one of {', '.join(map(repr, PRECISIONS))}, got {precision!r}")
         self.cfg = cfg
         self.name = name or cfg.name
         self.precision = precision
@@ -180,9 +213,17 @@ class Model:
     def act_dtype(self) -> torch.dtype:
         return torch.bfloat16 if self.precision == "bf16" else torch.float32
 
+    def _gemm_operand(self, w: torch.Tensor) -> torch.Tensor:
+        """A GEMM / convolution weight matrix as the kernels take it: in the activation dtype and, for tf32 models,
+        rounded to TF32 once here (the TF32 kernels round only their activation operand)."""
+        w = w.to(self.act_dtype)
+        if self.precision == "tf32":
+            w = _lib.round_tf32(w)
+        return w.contiguous()
+
     def _dense_weight(self, key: str, pad_k_to: int = 8) -> torch.Tensor:
         """TF Dense/Conv kernel ``(..., in, out)`` -> engine layout ``W[out][K]`` (K contiguous,
-        K = prod(leading dims), zero-padded to a multiple of ``pad_k_to``), in the activation dtype."""
+        K = prod(leading dims), zero-padded to a multiple of ``pad_k_to``), a GEMM operand (``_gemm_operand``)."""
         w = self.params[key]
         out = w.shape[-1]
         w2 = w.reshape(-1, out).t().contiguous()  # (out, K)
@@ -190,7 +231,7 @@ class Model:
         Kpad = (K + pad_k_to - 1) // pad_k_to * pad_k_to
         if Kpad != K:
             w2 = torch.nn.functional.pad(w2, (0, Kpad - K))
-        return w2.to(self.act_dtype).contiguous()
+        return self._gemm_operand(w2)
 
     def _vec(self, key: str) -> torch.Tensor:
         return self.params[key].reshape(-1).float().contiguous()
@@ -223,7 +264,7 @@ class Model:
             return x.to(self.device, non_blocking=True).contiguous()
         if x.dtype not in (torch.float32, torch.bfloat16):
             x = x.float()
-        if self.precision == "fp32" and x.dtype != torch.float32:
+        if self.precision != "bf16" and x.dtype != torch.float32:
             x = x.float()
         return x.to(self.device, non_blocking=True).contiguous()
 

@@ -21,9 +21,12 @@ ROOT = Path(__file__).resolve().parent.parent
 
 # kernel-name substring -> family name used by tfimm.backend.ops._call / bench.py
 FAMILIES = [
-    ("mlp_fused", "mlp_bf16"), ("gemm_bf16_wgmma", "gemm_bf16"), ("gemm_bf16_skinny", "gemm_bf16"),
+    ("mlp_fused", "mlp_bf16"),
+    # the TF32 instances of the wgmma GEMM (template argument A-transform = 2, fp32 out) before the bf16 ones
+    ("gemm_wgmma_kernelILi64EfLi2E", "gemm_tf32"), ("gemm_wgmma_kernelILi128EfLi2E", "gemm_tf32"),
+    ("gemm_wgmma", "gemm_bf16"), ("gemm_bf16_skinny", "gemm_bf16"),
     ("gemm_f32", "gemm_f32"),
-    ("vit_attention", "attention_bf16"), ("attention_cls", "attention_cls_bf16"), ("attention_f32", "attention_f32"),
+    ("vit_attention_tf32", "attention_tf32"), ("vit_attention", "attention_bf16"), ("attention_cls", "attention_cls_bf16"), ("attention_f32", "attention_f32"),
     ("window_attention", "window_attention_bf16"),
     ("layernorm_patch2x2", "layernorm_patch2x2"), ("patch_merge_ln", "patch_merge_ln"), ("layernorm", "layernorm"),
     ("dwconv7_ln", "dwconv_ln"), ("dwconv_ln", "dwconv_ln"), ("dwconv_act", "dwconv_bias_act"),
