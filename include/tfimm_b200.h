@@ -273,6 +273,29 @@ int tfimm_b200_eca_gate(const float* mean, const float* w, float* gate, int B, i
 int tfimm_b200_scale_add_act(void* x, int dtype, const float* gate, const void* shortcut, int B, int HW, int C,
                              int act, void* stream);
 
+/* Segment Anything image-encoder attention with decomposed relative-position terms, for global and windowed blocks:
+ * RelPosAttention.call + add_decomposed_rel_pos + window_partition / window_unpartition
+ * (tfimm/architectures/segment_anything/image_encoder.py:231-263, 121-168, 11-73).  Per image and head,
+ *     out_i = softmax_j(scale q_i . k_j + q_i . R_h[qy - ky + S_h - 1] + q_i . R_w[qx - kx + S_w - 1]) v_j
+ * with the UNSCALED q in the relative-position terms.  qkv: [B * gh * gw][3 * H * dh] of the real tokens (row-major over
+ * the gh x gw grid), column order [q | k | v] each head-major; out: [B * gh * gw][H * dh].
+ * window == 0: one sequence of S_h x S_w = gh x gw tokens.  window > 0: S x S windows of the grid zero-padded to a
+ * multiple of S; a padding position is a key with k = b_k and v = b_v taken from pad_bias ([3 * H * dh], the qkv bias;
+ * NULL: zero keys), as in the reference, where the padded rows of norm1's output are projected by the qkv Dense.
+ * Padding positions produce no output row.  rel_h: fp32 [2 S_h - 1][dh], rel_w: fp32 [2 S_w - 1][dh] (already resized
+ * to the sequence extent, get_rel_pos image_encoder.py:76-118).  S_h, S_w <= 127.  No N x N tensor is materialised.
+ * bf16: qkv / out / pad_bias bf16, dh 64 or 80, S_h + S_w <= 153 (dh 64) / <= 137 (dh 80) -- shared memory; other
+ * shapes: TFIMM_ERR_UNSUPPORTED --, 64-key blocks streamed through shared memory, mma.sync products, fp32 online
+ * softmax, P rounded to bf16 per block. */
+int tfimm_b200_relpos_attention_bf16(const void* qkv, void* out, const void* pad_bias, const float* rel_h,
+                                     const float* rel_w, int B, int gh, int gw, int H, int dh, int window, float scale,
+                                     void* stream);
+
+/* Same contract in fp32 on CUDA cores (precision="fp32"), any head_dim; S_h * S_w up to ~13k tokens. */
+int tfimm_b200_relpos_attention_f32(const float* qkv, float* out, const float* pad_bias, const float* rel_h,
+                                    const float* rel_w, int B, int gh, int gw, int H, int dh, int window, float scale,
+                                    void* stream);
+
 /* Elementwise dtype conversion. */
 int tfimm_b200_cast(const void* in, int in_dtype, void* out, int out_dtype, long n, void* stream);
 

@@ -93,6 +93,10 @@ int grouped_conv(const void*, int, const float*, const float*, void*, int, int, 
                  int, int, cudaStream_t);
 int eca_gate(const float*, const float*, float*, int, int, int, cudaStream_t);
 int scale_add_act(void*, int, const float*, const void*, int, int, int, int, cudaStream_t);
+int relpos_attention_bf16(const void*, void*, const void*, const float*, const float*, int, int, int, int, int, int,
+                          float, cudaStream_t);
+int relpos_attention_f32(const float*, float*, const float*, const float*, const float*, int, int, int, int, int, int,
+                         float, cudaStream_t);
 
 }  // namespace tfimm
 
@@ -289,6 +293,18 @@ int tfimm_b200_eca_gate(const float* mean, const float* w, float* gate, int B, i
 int tfimm_b200_scale_add_act(void* x, int dtype, const float* gate, const void* shortcut, int B, int HW, int C,
                              int act, void* stream) {
   return tfimm::scale_add_act(x, dtype, gate, shortcut, B, HW, C, act, S(stream));
+}
+
+int tfimm_b200_relpos_attention_bf16(const void* qkv, void* out, const void* pad_bias, const float* rel_h,
+                                     const float* rel_w, int B, int gh, int gw, int H, int dh, int window, float scale,
+                                     void* stream) {
+  return tfimm::relpos_attention_bf16(qkv, out, pad_bias, rel_h, rel_w, B, gh, gw, H, dh, window, scale, S(stream));
+}
+
+int tfimm_b200_relpos_attention_f32(const float* qkv, float* out, const float* pad_bias, const float* rel_h,
+                                    const float* rel_w, int B, int gh, int gw, int H, int dh, int window, float scale,
+                                    void* stream) {
+  return tfimm::relpos_attention_f32(qkv, out, pad_bias, rel_h, rel_w, B, gh, gw, H, dh, window, scale, S(stream));
 }
 
 }  // extern "C"

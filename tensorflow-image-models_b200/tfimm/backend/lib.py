@@ -60,6 +60,8 @@ SIGNATURES = {
     "tfimm_b200_grouped_conv": [_P, _I, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P],
     "tfimm_b200_eca_gate": [_P, _P, _P, _I, _I, _I, _P],
     "tfimm_b200_scale_add_act": [_P, _I, _P, _P, _I, _I, _I, _I, _P],
+    "tfimm_b200_relpos_attention_bf16": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _P],
+    "tfimm_b200_relpos_attention_f32": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _P],
 }
 _SPECIAL = {
     "tfimm_b200_version": ([], _c.c_char_p),

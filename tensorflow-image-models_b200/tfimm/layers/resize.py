@@ -46,6 +46,15 @@ def tf_bicubic_resize(images: torch.Tensor, size: Tuple[int, int]) -> torch.Tens
     return torch.einsum("pw,bowc->bopc", mw, out)
 
 
+def tf_bilinear_resize(images: torch.Tensor, size: Tuple[int, int]) -> torch.Tensor:
+    """``tf.image.resize(images, size, method="bilinear")`` for NHWC tensors (``antialias=False``: the ResizeBilinear op
+    with ``half_pixel_centers=True``, source coordinate ``(o + 0.5) * scale - 0.5`` clamped to the image), which is
+    PyTorch's ``align_corners=False`` bilinear interpolation."""
+    x = torch.nn.functional.interpolate(images.permute(0, 3, 1, 2), size=tuple(size), mode="bilinear",
+                                        align_corners=False)
+    return x.permute(0, 2, 3, 1).contiguous()
+
+
 def interpolate_pos_embeddings(pos_embed: torch.Tensor, src_grid_size, tgt_grid_size, nb_tokens: int = 0):
     """(1, nb_tokens + h*w, D) -> (1, nb_tokens + h'*w', D); token embeddings are kept as they are."""
     src_grid_size, tgt_grid_size = tuple(src_grid_size), tuple(tgt_grid_size)

@@ -26,6 +26,8 @@ FAMILIES = [
     ("gemm_wgmma_kernelILi64EfLi2E", "gemm_tf32"), ("gemm_wgmma_kernelILi128EfLi2E", "gemm_tf32"),
     ("gemm_wgmma", "gemm_bf16"), ("gemm_bf16_skinny", "gemm_bf16"),
     ("gemm_f32", "gemm_f32"),
+    # before "attention_f32": the Segment Anything kernels' names contain it
+    ("relpos_attention_bf16", "relpos_attention_bf16"), ("relpos_attention_f32", "relpos_attention_f32"),
     ("vit_attention_tf32", "attention_tf32"), ("vit_attention", "attention_bf16"), ("attention_cls", "attention_cls_bf16"), ("attention_f32", "attention_f32"),
     ("window_attention", "window_attention_bf16"),
     ("layernorm_patch2x2", "layernorm_patch2x2"), ("patch_merge_ln", "patch_merge_ln"), ("layernorm", "layernorm"),
