@@ -296,6 +296,47 @@ int tfimm_b200_relpos_attention_f32(const float* qkv, float* out, const float* p
                                     const float* rel_w, int B, int gh, int gw, int H, int dh, int window, float scale,
                                     void* stream);
 
+/* ---- MLP-Mixer family (MLP-Mixer, gMixer, ResMLP, gMLP) ----
+ * Token mixing: a Dense layer applied along the token axis of a transposed activation -- `transpose -> Dense ->
+ * transpose` of MixerBlock.call's mlp_tokens (tfimm/architectures/mlp_mixer.py:115-121), ResBlock.linear_tokens
+ * (mlp_mixer.py:175-181) and SpatialGatingUnit.proj (tfimm/layers/transformers.py:376-383) -- without the transposes:
+ *     out[b][m][c] = epi(sum_n Wt[m][n] X[b][n][c]),   b < imgs, m < M (rows of Wt), n < K (tokens in), c < N
+ * Wt: bf16 [M][K], K-major, row stride ldw (a multiple of 8: the Dense kernel transposed and padded at plan time).
+ * X: bf16, row stride ldx and image stride img_x (multiples of 8 elements), read where it is stored (MN-major wgmma
+ * operand; a strided view such as gMLP's normalised v half works).  Epilogue, in this order:
+ *   + bias[m] (per output ROW)  -> act, or with glu: rows come in groups of 16 (8 value rows, then their 8 gate rows)
+ *   and stored row 8 (m / 16) + m % 8 is value * act(gate)  -> * gamma[c]  -> * mul[b][row][c] (gMLP's u half;
+ *   row stride ld_mul, image stride img_mul)  -> + residual[b][row][c] (may alias out)  -> store at
+ *   out + b * img_c + row * ldc + c.  Rows >= m_out are not stored.  out / residual / mul: out_dtype (bf16 / fp32).
+ * force_block_n: 0 = auto; 64 / 128 / 256 = that tile width. */
+int tfimm_b200_token_gemm_bf16(const void* Wt, int ldw, const void* X, long ldx, long img_x, const float* bias,
+                               const float* gamma, const void* residual, long ldr, long img_r, const void* mul,
+                               long ld_mul, long img_mul, void* out, long ldc, long img_c, int imgs, int M, int N, int K,
+                               int m_out, int act, int glu, int out_dtype, int force_block_n, void* stream);
+
+/* Same contract in fp32 on CUDA cores (precision="fp32"); ldw >= K, no alignment requirements. */
+int tfimm_b200_token_gemm_f32(const float* Wt, int ldw, const float* X, long ldx, long img_x, const float* bias,
+                              const float* gamma, const float* residual, long ldr, long img_r, const float* mul,
+                              long ld_mul, long img_mul, float* out, long ldc, long img_c, int imgs, int M, int N, int K,
+                              int m_out, int act, int glu, void* stream);
+
+/* Channel GLU: GluMLP's fc1 + split + x * act(gates) (tfimm/layers/transformers.py:345-348, gMixer's mlp_channels) in
+ * one GEMM.  W: bf16 [N][K] whose rows 2j / 2j + 1 are value / gate feature j (interleaved at plan time), bias [N]
+ * likewise; out: bf16 [M][N / 2], row stride ldc = (value + bias) * act(gate + bias).  The full-width hidden tensor
+ * is never written. */
+int tfimm_b200_gemm_glu_bf16(const void* A, int lda, const void* W, int ldw, const float* bias, void* C, int ldc, int M,
+                             int N, int K, int act, int force_block_n, void* stream);
+
+/* fp32 form of the channel GLU on CUDA cores: W rows in the token GEMM's pairing (per 16 rows: 8 value features, then
+ * their 8 gates; N % 16 == 0), out: fp32 [M][n_out]. */
+int tfimm_b200_gemm_glu_f32(const float* A, int lda, const float* W, int ldw, const float* bias, float* C, int ldc,
+                            int M, int N, int n_out, int K, int act, void* stream);
+
+/* ResMLP's Affine norm (tfimm/layers/norm.py:32-34): out[r][c] = alpha[c] * x[r][c] + beta[c]; fp32 x (row stride
+ * ldx), out bf16 / fp32 (row stride ldo). */
+int tfimm_b200_affine(const float* x, long ldx, const float* alpha, const float* beta, void* out, int out_dtype,
+                      long ldo, long rows, int C, void* stream);
+
 /* Elementwise dtype conversion. */
 int tfimm_b200_cast(const void* in, int in_dtype, void* out, int out_dtype, long n, void* stream);
 

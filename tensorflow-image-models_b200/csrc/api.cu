@@ -98,6 +98,16 @@ int relpos_attention_bf16(const void*, void*, const void*, const float*, const f
 int relpos_attention_f32(const float*, float*, const float*, const float*, const float*, int, int, int, int, int, int,
                          float, cudaStream_t);
 
+int token_gemm_bf16_dispatch(const void*, int, const void*, long, long, const float*, const float*, const void*, long,
+                             long, const void*, long, long, void*, long, long, int, int, int, int, int, int, int, int,
+                             int, cudaStream_t);
+int token_gemm_f32(const float*, int, const float*, long, long, const float*, const float*, const float*, long, long,
+                   const float*, long, long, float*, long, long, int, int, int, int, int, int, int, cudaStream_t);
+int gemm_glu_bf16_dispatch(const void*, int, const void*, int, const float*, void*, int, int, int, int, int, int,
+                           cudaStream_t);
+int gemm_glu_f32(const float*, int, const float*, int, const float*, float*, int, int, int, int, int, int, cudaStream_t);
+int affine(const float*, long, const float*, const float*, void*, int, long, long, int, cudaStream_t);
+
 }  // namespace tfimm
 
 using tfimm::set_last_error;
@@ -308,3 +318,35 @@ int tfimm_b200_relpos_attention_f32(const float* qkv, float* out, const float* p
 }
 
 }  // extern "C"
+
+int tfimm_b200_token_gemm_bf16(const void* Wt, int ldw, const void* X, long ldx, long img_x, const float* bias,
+                               const float* gamma, const void* residual, long ldr, long img_r, const void* mul,
+                               long ld_mul, long img_mul, void* out, long ldc, long img_c, int imgs, int M, int N, int K,
+                               int m_out, int act, int glu, int out_dtype, int force_block_n, void* stream) {
+  return tfimm::token_gemm_bf16_dispatch(Wt, ldw, X, ldx, img_x, bias, gamma, residual, ldr, img_r, mul, ld_mul, img_mul,
+                                         out, ldc, img_c, imgs, M, N, K, m_out, act, glu, out_dtype, force_block_n,
+                                         S(stream));
+}
+
+int tfimm_b200_token_gemm_f32(const float* Wt, int ldw, const float* X, long ldx, long img_x, const float* bias,
+                              const float* gamma, const float* residual, long ldr, long img_r, const float* mul,
+                              long ld_mul, long img_mul, float* out, long ldc, long img_c, int imgs, int M, int N, int K,
+                              int m_out, int act, int glu, void* stream) {
+  return tfimm::token_gemm_f32(Wt, ldw, X, ldx, img_x, bias, gamma, residual, ldr, img_r, mul, ld_mul, img_mul, out, ldc,
+                               img_c, imgs, M, N, K, m_out, act, glu, S(stream));
+}
+
+int tfimm_b200_gemm_glu_bf16(const void* A, int lda, const void* W, int ldw, const float* bias, void* C, int ldc, int M,
+                             int N, int K, int act, int force_block_n, void* stream) {
+  return tfimm::gemm_glu_bf16_dispatch(A, lda, W, ldw, bias, C, ldc, M, N, K, act, force_block_n, S(stream));
+}
+
+int tfimm_b200_gemm_glu_f32(const float* A, int lda, const float* W, int ldw, const float* bias, float* C, int ldc,
+                            int M, int N, int n_out, int K, int act, void* stream) {
+  return tfimm::gemm_glu_f32(A, lda, W, ldw, bias, C, ldc, M, N, n_out, K, act, S(stream));
+}
+
+int tfimm_b200_affine(const float* x, long ldx, const float* alpha, const float* beta, void* out, int out_dtype,
+                      long ldo, long rows, int C, void* stream) {
+  return tfimm::affine(x, ldx, alpha, beta, out, out_dtype, ldo, rows, C, S(stream));
+}

@@ -476,6 +476,20 @@ __device__ __forceinline__ uint64_t gmma_desc_k_sw128(uint32_t smem_addr) {
   d |= (uint64_t)1 << 62;
   return d;
 }
+// Descriptor for an MN-major bf16 B tile (wgmma imm-trans-b = 1) written by TMA SWIZZLE_128B as boxes of 64 MN
+// elements (one 128-byte span) x 64 K rows: every K row is a 128-byte span, the swizzle atom is 64 MN x 8 K (1024 B).
+// Here the two offsets mean something else than in the K-major form:
+//   leading byte offset = stride between 64-element MN atoms (the next TMA box: 64 rows * 128 B = 8192)
+//   stride byte offset  = stride between 8-row K groups (1024)
+// Advancing 16 elements along K is 16 rows = 2048 bytes, i.e. +128 on the descriptor.
+__device__ __forceinline__ uint64_t gmma_desc_mn_sw128(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
+  d |= (uint64_t)(8192 >> 4) << 16;
+  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)1 << 62;
+  return d;
+}
 // ---- thread-block clusters ----
 __device__ __forceinline__ void cluster_arrive_release() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");

@@ -34,6 +34,17 @@ struct GemmParams {
   int cv_pb, cv_ph, cv_pw;
   int cv_tiles_x, cv_tiles_y;  // patch grid per image group (x fastest, then y, then image group)
   int cv_B, cv_Ho, cv_Wo;
+  // Token mixing (gemm_sm90.cu, kModeToken) and the channel GLU (kModeGluCols).  Token mixing: the tile grid is
+  // images x (M / 128) x (N / BLOCK_N); A is the transposed Dense kernel Wt[M][K] (K = tokens in), B the activation
+  // X[image][K][N] read MN-major, and output row m of image b lives at b * img_c + m * ldc (residual: img_r, ldr).
+  // bias is per output ROW; rows >= m_out are not stored.  glu: A rows come in groups of 16 -- 8 value rows, then
+  // their 8 gate rows -- and stored row 8 (m / 16) + m % 8 is value * act(gate) (kModeGluCols: columns 2j, 2j + 1 are
+  // value and gate of stored column j).  mul: elementwise multiplier in the output's element type (the gMLP gate's u
+  // half), row stride ld_mul and image stride img_mul.
+  int tk_imgs, m_out, glu;
+  long img_c, img_r;
+  const void* mul;
+  long ld_mul, img_mul;
 };
 
 // Element offset of output row `r` (0..127) of tile m_blk, or -1 when the row lies outside the output.
@@ -155,6 +166,80 @@ __device__ __forceinline__ void epilogue_frag(const GemmParams& p, float (&acc)[
 #pragma unroll
     for (int h = 0; h < 2; ++h)
       if (in && off_c[h] >= 0) st_out_pair(C + off_c[h] + n, v[h], two);
+  }
+}
+
+// Epilogue of the token-mixing GEMM (kModeToken): one warpgroup's 64 x BN accumulator of tile (img, m_blk, n_blk).
+// Per element: acc + bias[row] -> act (glu: value * act(gate)) -> * gamma[col] -> * mul -> + residual -> store.
+template <typename OutT, int BN>
+__device__ __forceinline__ void epilogue_token(const GemmParams& p, float (&acc)[BN / 2], int img, int m_blk, int n_blk,
+                                               int wg_row0) {
+  const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
+  const int m0 = m_blk * 128 + wg_row0 + wq * 16 + (lane >> 2);   // A rows m0 and m0 + 8 (m0 % 16 < 8)
+  const float b0 = p.bias != nullptr && m0 < p.M ? __ldg(p.bias + m0) : 0.f;
+  const float b1 = p.bias != nullptr && m0 + 8 < p.M ? __ldg(p.bias + m0 + 8) : 0.f;
+  // stored rows: (m0, m0 + 8), or the one GLU row
+  const int rows[2] = {p.glu ? (m0 >> 4) * 8 + (m0 & 7) : m0, p.glu ? -1 : m0 + 8};
+  OutT* __restrict__ C = reinterpret_cast<OutT*>(p.c) + (long)img * p.img_c;
+  const OutT* R = reinterpret_cast<const OutT*>(p.res) + (long)img * p.img_r;
+  const OutT* U = reinterpret_cast<const OutT*>(p.mul) + (long)img * p.img_mul;
+#pragma unroll
+  for (int g = 0; g < BN / 8; ++g) {
+    const int n = n_blk * BN + g * 8 + 2 * (lane & 3);
+    if (n_blk * BN + g * 8 >= p.N) break;
+    const bool in = n < p.N, two = n + 1 < p.N;
+    uint64_t v[2] = {pack2(acc[4 * g + 0] + b0, acc[4 * g + 1] + b0), pack2(acc[4 * g + 2] + b1, acc[4 * g + 3] + b1)};
+    if (p.glu) {
+      float x0, x1, g0, g1;
+      unpack2(v[0], x0, x1);
+      unpack2(v[1], g0, g1);
+      v[0] = pack2(x0 * apply_act<false>(g0, p.act), x1 * apply_act<false>(g1, p.act));
+    } else {
+      apply_act_pairs(v, p.act);
+    }
+    if (p.gamma != nullptr) {
+      const uint64_t s = ld_pair_or(p.gamma, n, p.N, 1.f);
+      v[0] = mul2(v[0], s);
+      v[1] = mul2(v[1], s);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = rows[h];
+      if (!in || row < 0 || row >= p.m_out) continue;
+      if (p.mul != nullptr) v[h] = mul2(v[h], ld_out_pair(U + (long)row * p.ld_mul + n, two));
+      if (p.has_res) v[h] = add2(v[h], ld_out_pair(R + (long)row * p.ldr + n, two));
+      st_out_pair(C + (long)row * p.ldc + n, v[h], two);
+    }
+  }
+}
+
+// Epilogue of the channel GLU GEMM (kModeGluCols): accumulator columns 2j / 2j + 1 are value / gate of output column
+// j, so each thread holds both halves of its pairs; stored: (value + bias) * act(gate + bias) at half width.
+template <typename OutT, int BN>
+__device__ __forceinline__ void epilogue_glu_cols(const GemmParams& p, float (&acc)[BN / 2], int m_blk, int n_blk,
+                                                  int wg_row0) {
+  const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
+  const int r = wg_row0 + wq * 16 + (lane >> 2);
+  const long off_c[2] = {epilogue_row_offset(p, m_blk, r, p.ldc), epilogue_row_offset(p, m_blk, r + 8, p.ldc)};
+  OutT* __restrict__ C = reinterpret_cast<OutT*>(p.c);
+#pragma unroll
+  for (int g = 0; g < BN / 8; ++g) {
+    const int n = n_blk * BN + g * 8 + 2 * (lane & 3);   // even: (value, gate) of output column n / 2
+    if (n_blk * BN + g * 8 >= p.N) break;
+    if (n >= p.N) continue;
+    float bx = 0.f, bg = 0.f;
+    if (p.bias != nullptr) {
+      const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+      bx = b.x; bg = b.y;
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (off_c[h] < 0) continue;
+      const float x = acc[4 * g + 2 * h] + bx, gt = acc[4 * g + 2 * h + 1] + bg;
+      const float y = x * apply_act<false>(gt, p.act);
+      if constexpr (sizeof(OutT) == 2) C[off_c[h] + n / 2] = __float2bfloat16_rn(y);
+      else C[off_c[h] + n / 2] = y;
+    }
   }
 }
 

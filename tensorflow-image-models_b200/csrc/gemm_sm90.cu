@@ -17,6 +17,14 @@
 //   warps 9..12 (A-transform instances only) rewrite the A tile in smem before the MMA reads it: the squeeze-excite
 //               gate (bf16), or the TF32 rounding of fp32 activations (precision="tf32")
 //
+// Two more instances share the ring, barriers, producer/consumer split and epilogue plumbing (GemmMode):
+//   kModeToken   token mixing, out[b][m][c] = epi(sum_n Wt[m][n] X[b][n][c]): the Dense layer that MLP-Mixer, ResMLP
+//                and gMLP apply along the token axis of a transposed activation.  B is X where it is stored, read
+//                MN-major (channels contiguous) as 3-D TMA boxes {64 channels, 64 tokens, 1 image} and fed to wgmma with
+//                imm-trans-b = 1; the token axis is a bounded TMA dimension, so the K tail reads zeros and no tile
+//                reads the next image.  Epilogue: epilogue_token (row bias, GLU on row pairs, multiplier).
+//   kModeGluCols a plain GEMM whose epilogue writes value * act(gate) of interleaved column pairs at half width.
+//
 // Operands: bf16 (wgmma k16), or fp32 rounded to TF32 (wgmma k8).  Either way a tile row is 128 bytes -- one
 // SWIZZLE_128B span of 64 bf16 or 32 fp32 contraction indices -- so stage bytes, descriptors and the 32-byte k-step are
 // the same; only the TMA element type, the k-block width and the MMA instruction differ.
@@ -41,6 +49,8 @@ enum ATransform : int {
   kAGate = 1,   // bf16 A: x * gate[image][k] in fp32, rounded back to bf16 (squeeze-excite)
   kATf32 = 2,   // fp32 A: cvt.rna.tf32 of every element (precision="tf32")
 };
+enum GemmMode : int { kModeGemm = 0, kModeToken = 1, kModeGluCols = 2 };
+
 template <int AX>
 using OperandT = std::conditional_t<AX == kATf32, float, __nv_bfloat16>;
 template <int AX>
@@ -58,10 +68,19 @@ struct GemmCfg {
   static constexpr int kSmemBytes = kStages * kStageBytes + kNumBarriers * 8 + 1024 /*alignment slack*/;
 };
 
+// B operand descriptor: K-major, or MN-major for token mixing; one k16 step is 32 bytes (+2) or 16 MN-major rows (+128).
+template <bool kMN>
+__device__ __forceinline__ uint64_t gmma_desc_b(uint32_t smem_addr) {
+  if constexpr (kMN) return gmma_desc_mn_sw128(smem_addr);
+  else return gmma_desc_k_sw128(smem_addr);
+}
+template <bool kMN>
+constexpr int kDescStepB = kMN ? 128 : 2;
+
 template <int BLOCK_N, int AX>
 constexpr int gemm_threads() { return kConsumerThreads + 32 + (AX != kANone ? 32 * kNumGateWarps : 0); }
 
-template <int BLOCK_N, typename OutT, int AX = kANone>
+template <int BLOCK_N, typename OutT, int AX = kANone, int MODE = kModeGemm>
 __global__ void __launch_bounds__(gemm_threads<BLOCK_N, AX>(), (BLOCK_N == 64 && AX == kANone) ? 2 : 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                        const GemmParams p) {
@@ -94,7 +113,16 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   __syncthreads();
 
   const int num_n_tiles = (p.N + BLOCK_N - 1) / BLOCK_N;
-  const int m_blk = blockIdx.x / num_n_tiles, n_blk = blockIdx.x % num_n_tiles;
+  int m_blk, n_blk, img = 0;
+  if constexpr (MODE == kModeToken) {
+    // token mixing: image-major tile order, tiles never cross images
+    const int img_tiles = ((p.M + kBlockM - 1) / kBlockM) * num_n_tiles;
+    img = (int)blockIdx.x / img_tiles;
+    const int tile = (int)blockIdx.x - img * img_tiles;
+    m_blk = tile / num_n_tiles; n_blk = tile % num_n_tiles;
+  } else {
+    m_blk = blockIdx.x / num_n_tiles; n_blk = blockIdx.x % num_n_tiles;
+  }
   const int num_k_blocks = (p.K + kBlockK - 1) / kBlockK;
 
   if (warp_idx == kProducerWarp) {
@@ -118,7 +146,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
           tma_load_4d(sa, &tmap_a, full_bar(stage), cb * kBlockK, tx * p.cv_pw * p.cv_stride + kx - p.cv_pad,
                       ty * p.cv_ph * p.cv_stride + ky - p.cv_pad, tb * p.cv_pb);
         }
-        tma_load_2d(sb, &tmap_b, full_bar(stage), kb * kBlockK, n_blk * BLOCK_N);
+        if constexpr (MODE == kModeToken) {
+#pragma unroll
+          for (int i = 0; i < BLOCK_N / 64; ++i)
+            tma_load_3d(sb + i * 8192, &tmap_b, full_bar(stage), n_blk * BLOCK_N + i * 64, kb * kBlockK, img);
+        } else {
+          tma_load_2d(sb, &tmap_b, full_bar(stage), kb * kBlockK, n_blk * BLOCK_N);
+        }
         if (++stage == kStages) { stage = 0; phase ^= 1u; }
       }
     }
@@ -233,7 +267,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       mbar_wait(AX != kANone ? ready_bar(stage) : full_bar(stage), phase);
       const uint32_t sa = smem_tiles + stage * Cfg::kStageBytes;
       const uint64_t da = gmma_desc_k_sw128(sa + (uint32_t)wg * (64 * 128));
-      const uint64_t db = gmma_desc_k_sw128(sa + Cfg::kABytes);
+      const uint64_t db = gmma_desc_b<MODE == kModeToken>(sa + Cfg::kABytes);
       wgmma_fence();
       // four 32-byte k-steps per 128-byte row (k16 bf16 / k8 tf32): +2 on the descriptors each
 #pragma unroll
@@ -241,7 +275,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         if constexpr (AX == kATf32)
           wgmma_ss_tf32<BLOCK_N>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (uint32_t)((kb | k) != 0));
         else
-          wgmma_ss<BLOCK_N>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (uint32_t)((kb | k) != 0));
+          wgmma_ss<BLOCK_N, MODE == kModeToken>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(kDescStepB<MODE == kModeToken> * k),
+                                                (uint32_t)((kb | k) != 0));
       }
       wgmma_commit();
       // the group issued one k-block ago has retired: its stage may be refilled
@@ -252,7 +287,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     }
     wgmma_wait<0>();
     if (releaser) mbar_arrive(empty_bar(prev));
-    epilogue_frag<OutT, BLOCK_N>(p, acc, m_blk, n_blk, wg * 64);
+    if constexpr (MODE == kModeToken) epilogue_token<OutT, BLOCK_N>(p, acc, img, m_blk, n_blk, wg * 64);
+    else if constexpr (MODE == kModeGluCols) epilogue_glu_cols<OutT, BLOCK_N>(p, acc, m_blk, n_blk, wg * 64);
+    else epilogue_frag<OutT, BLOCK_N>(p, acc, m_blk, n_blk, wg * 64);
   }
 }
 
@@ -266,7 +303,7 @@ int check_out(const void* C, long ldc, const void* residual, long ldr, int esize
   return kOk;
 }
 
-template <int BLOCK_N, typename OutT, int AX = kANone>
+template <int BLOCK_N, typename OutT, int AX = kANone, int MODE = kModeGemm>
 int launch_gemm(const void* A, int lda, const void* W, int ldw, const void* residual, int ldr, void* C, int ldc,
                 GemmParams p, cudaStream_t stream) {
   const int M = p.M, N = p.N, K = p.K;
@@ -278,18 +315,45 @@ int launch_gemm(const void* A, int lda, const void* W, int ldw, const void* resi
   if ((st = make_tmap_2d(&ta, A, dtype_code<AX>(), M, K, lda, kBlockM, kBlockK, "A")) != kOk) return st;
   if ((st = make_tmap_2d(&tb, W, dtype_code<AX>(), N, K, ldw, BLOCK_N, kBlockK, "W")) != kOk) return st;
   p.c = C; p.res = residual; p.ldc = ldc; p.ldr = ldr;
-  auto kernel = gemm_wgmma_kernel<BLOCK_N, OutT, AX>;
+  auto kernel = gemm_wgmma_kernel<BLOCK_N, OutT, AX, MODE>;
   static unsigned long long attr_devs = 0;  // per instantiation
   if (first_use_on_device(attr_devs)) {
     TFIMM_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
   }
   const long tiles = (long)((M + kBlockM - 1) / kBlockM) * ((N + BLOCK_N - 1) / BLOCK_N);
   kernel<<<(unsigned)tiles, gemm_threads<BLOCK_N, AX>(), Cfg::kSmemBytes, stream>>>(ta, tb, p);
-  TFIMM_LAUNCH_OK(AX == kATf32 ? "gemm_wgmma_kernel (tf32)" : "gemm_wgmma_kernel (bf16)");
+  TFIMM_LAUNCH_OK(AX == kATf32 ? "gemm_wgmma_kernel (tf32)"
+                               : (MODE == kModeGluCols ? "gemm_wgmma_kernel (bf16 glu)" : "gemm_wgmma_kernel (bf16)"));
   return kOk;
 }
 
 int pick_block_n(int M, int N);
+
+// Token mixing (kModeToken): A = Wt[M][K] (K-major, row stride ldw), B = X[imgs][K][N] (row stride ldx, image stride
+// img_x), both bf16.
+template <int BLOCK_N, typename OutT>
+int launch_token(const void* Wt, int ldw, const void* X, long ldx, long img_x, GemmParams p, cudaStream_t stream) {
+  using Cfg = GemmCfg<BLOCK_N>;
+  CUtensorMap ta, tb;
+  int st;
+  if ((st = check_out(p.c, p.ldc, p.res, p.ldr, (int)sizeof(OutT))) != kOk) return st;
+  if ((st = make_tmap_2d(&ta, Wt, kBF16, p.M, p.K, ldw, kBlockM, 64, "token Wt")) != kOk) return st;
+  {
+    const uint64_t dims[3] = {(uint64_t)p.N, (uint64_t)p.K, (uint64_t)p.tk_imgs};
+    const uint64_t strides[2] = {(uint64_t)ldx * 2, (uint64_t)img_x * 2};
+    const uint32_t box[3] = {64u, 64u, 1u};
+    if ((st = make_tmap(&tb, X, kBF16, 3, dims, strides, box, "token X")) != kOk) return st;
+  }
+  auto kernel = gemm_wgmma_kernel<BLOCK_N, OutT, kANone, kModeToken>;
+  static unsigned long long attr_devs = 0;  // per instantiation
+  if (first_use_on_device(attr_devs)) {
+    TFIMM_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+  }
+  const long tiles = (long)p.tk_imgs * ((p.M + kBlockM - 1) / kBlockM) * ((p.N + BLOCK_N - 1) / BLOCK_N);
+  kernel<<<(unsigned)tiles, gemm_threads<BLOCK_N, kANone>(), Cfg::kSmemBytes, stream>>>(ta, tb, p);
+  TFIMM_LAUNCH_OK("gemm_wgmma_kernel (bf16 token mixing)");
+  return kOk;
+}
 
 // Implicit k x k convolution on the tensor cores: same kernel, A tensor map = the NHWC input (rank 4, traversal
 // stride = conv stride), C / residual = the NHWC output.  See GemmParams::conv.
@@ -496,6 +560,73 @@ int conv_tf32_dispatch(const float* x, const float* W, int ldw, const float* bia
     return st;
   if (N >= 128) return launch_conv<128, float, kATf32>(x, W, ldw, residual, out, B, H, Wd, C, Ho, Wo, p, stream);
   return launch_conv<64, float, kATf32>(x, W, ldw, residual, out, B, H, Wd, C, Ho, Wo, p, stream);
+}
+
+// ---- MLP-Mixer family (tfimm.backend.mixer_ops) ----
+// Token mixing: out[b][m][c] = epi(sum_n Wt[m][n] X[b][n][c]), see GemmParams (kModeToken) for the epilogue.
+// Wt: bf16 [M][K], row stride ldw % 8 == 0 (rows padded at plan time); X: bf16, row stride ldx and image stride img_x,
+// both multiples of 8 elements.  out / residual / mul: bf16 or fp32 (out_dtype), rows of N elements.
+int token_gemm_bf16_dispatch(const void* Wt, int ldw, const void* X, long ldx, long img_x, const float* bias,
+                             const float* gamma, const void* residual, long ldr, long img_r, const void* mul, long ld_mul,
+                             long img_mul, void* out, long ldc, long img_c, int imgs, int M, int N, int K, int m_out,
+                             int act, int glu, int out_dtype, int force_block_n, cudaStream_t stream) {
+  TFIMM_CHECK_ARG(imgs > 0 && M > 0 && N > 0 && K > 0 && m_out > 0, "token_gemm: empty shape (imgs %d M %d N %d K %d)",
+                  imgs, M, N, K);
+  TFIMM_CHECK_ARG(out_dtype == kBF16 || out_dtype == kF32, "token_gemm: out_dtype must be bf16 or f32");
+  TFIMM_CHECK_ARG(ldw % 8 == 0 && ldw >= K && ldx % 8 == 0 && img_x % 8 == 0 && ldx >= N,
+                  "token_gemm: Wt / X strides must be multiples of 8 elements");
+  TFIMM_CHECK_ARG(glu ? (M % 16 == 0 && m_out <= M / 2) : m_out <= M, "token_gemm: m_out %d does not fit M %d (glu %d)",
+                  m_out, M, glu);
+  TFIMM_CHECK_ARG(N % 2 == 0 && (gamma == nullptr || (reinterpret_cast<uintptr_t>(gamma) & 7u) == 0),
+                  "token_gemm: N must be even and gamma 8-byte aligned");
+  const int es = out_dtype == kBF16 ? 2 : 4;
+  TFIMM_CHECK_ARG(mul == nullptr || ((reinterpret_cast<uintptr_t>(mul) & 15u) == 0 && (ld_mul * es) % 16 == 0 &&
+                                     (img_mul * es) % 16 == 0),
+                  "token_gemm: mul must be 16-byte aligned with strides of multiples of 16 bytes");
+  TFIMM_CHECK_ARG((img_c * es) % 16 == 0 && (residual == nullptr || (img_r * es) % 16 == 0),
+                  "token_gemm: image strides must be multiples of 16 bytes");
+  GemmParams p{};
+  p.M = M; p.N = N; p.K = K;
+  p.bias = bias; p.gamma = gamma; p.act = act; p.has_res = residual != nullptr ? 1 : 0;
+  p.c = out; p.res = residual; p.ldc = ldc; p.ldr = ldr;
+  p.tk_imgs = imgs; p.m_out = m_out; p.glu = glu; p.img_c = img_c; p.img_r = img_r;
+  p.mul = mul; p.ld_mul = ld_mul; p.img_mul = img_mul;
+  const int bn = force_block_n > 0 ? force_block_n : pick_block_n(imgs * ((M + kBlockM - 1) / kBlockM) * kBlockM, N);
+#define TFIMM_TOKEN_CASE(BN)                                                                              \
+  case BN:                                                                                                \
+    return out_dtype == kBF16 ? launch_token<BN, __nv_bfloat16>(Wt, ldw, X, ldx, img_x, p, stream)       \
+                              : launch_token<BN, float>(Wt, ldw, X, ldx, img_x, p, stream);
+  switch (bn) {
+    TFIMM_TOKEN_CASE(256)
+    TFIMM_TOKEN_CASE(128)
+    TFIMM_TOKEN_CASE(64)
+    default:
+      set_last_error("token_gemm: unsupported block_n %d", bn);
+      return kInvalidArgument;
+  }
+#undef TFIMM_TOKEN_CASE
+}
+
+// Channel GLU (gMixer's mlp_channels fc1): W rows 2j / 2j + 1 are value / gate feature j (interleaved at plan time),
+// bias likewise; out[M][N / 2] = (A W_value^T + b) * act(A W_gate^T + b), bf16.  The full-width hidden tensor is never
+// written.
+int gemm_glu_bf16_dispatch(const void* A, int lda, const void* W, int ldw, const float* bias, void* C, int ldc, int M,
+                           int N, int K, int act, int force_block_n, cudaStream_t stream) {
+  TFIMM_CHECK_ARG(M > 0 && N > 0 && K > 0 && K % 8 == 0 && N % 2 == 0,
+                  "gemm_glu: need K %% 8 == 0 and an even N (got M=%d N=%d K=%d)", M, N, K);
+  TFIMM_CHECK_ARG(bias == nullptr || (reinterpret_cast<uintptr_t>(bias) & 7u) == 0, "gemm_glu: bias must be 8-byte aligned");
+  GemmParams p{};
+  p.M = M; p.N = N; p.K = K;
+  p.bias = bias; p.act = act;
+  const int bn = force_block_n > 0 ? force_block_n : pick_block_n(M, N);
+  switch (bn) {
+    case 256: return launch_gemm<256, __nv_bfloat16, kANone, kModeGluCols>(A, lda, W, ldw, nullptr, 0, C, ldc, p, stream);
+    case 128: return launch_gemm<128, __nv_bfloat16, kANone, kModeGluCols>(A, lda, W, ldw, nullptr, 0, C, ldc, p, stream);
+    case 64: return launch_gemm<64, __nv_bfloat16, kANone, kModeGluCols>(A, lda, W, ldw, nullptr, 0, C, ldc, p, stream);
+    default:
+      set_last_error("gemm_glu: unsupported block_n %d", bn);
+      return kInvalidArgument;
+  }
 }
 
 }  // namespace tfimm

@@ -62,6 +62,13 @@ SIGNATURES = {
     "tfimm_b200_scale_add_act": [_P, _I, _P, _P, _I, _I, _I, _I, _P],
     "tfimm_b200_relpos_attention_bf16": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _P],
     "tfimm_b200_relpos_attention_f32": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _P],
+    "tfimm_b200_token_gemm_bf16": [_P, _I, _P, _L, _L, _P, _P, _P, _L, _L, _P, _L, _L, _P, _L, _L, _I, _I, _I, _I,
+                                   _I, _I, _I, _I, _I, _P],
+    "tfimm_b200_token_gemm_f32": [_P, _I, _P, _L, _L, _P, _P, _P, _L, _L, _P, _L, _L, _P, _L, _L, _I, _I, _I, _I,
+                                  _I, _I, _I, _P],
+    "tfimm_b200_gemm_glu_bf16": [_P, _I, _P, _I, _P, _P, _I, _I, _I, _I, _I, _I, _P],
+    "tfimm_b200_gemm_glu_f32": [_P, _I, _P, _I, _P, _P, _I, _I, _I, _I, _I, _I, _P],
+    "tfimm_b200_affine": [_P, _L, _P, _P, _P, _I, _L, _L, _I, _P],
 }
 _SPECIAL = {
     "tfimm_b200_version": ([], _c.c_char_p),

@@ -3,7 +3,7 @@
 The reference cannot be imported normally here (TensorFlow is not installed), but its config
 dataclasses and ``@register_model`` entry points are plain Python.  This script imports
 ``/root/reference/tfimm`` against a stub ``tensorflow`` module (every attribute is an inert
-class), reads the populated registry and writes, for the five in-scope families,
+class), reads the populated registry and writes, for the in-scope families,
 
     tensorflow-image-models_b200/tfimm/architectures/zoo/<family>.json
         {"<model name>": {<config field>: <value>, ...}, ...}
@@ -20,7 +20,7 @@ from pathlib import Path
 
 REFERENCE = Path("/root/reference")
 OUT = Path(__file__).resolve().parent.parent / "tensorflow-image-models_b200" / "tfimm" / "architectures" / "zoo"
-FAMILIES = ["vit", "swin", "convnext", "efficientnet", "resnet"]
+FAMILIES = ["vit", "swin", "convnext", "efficientnet", "resnet", "mlp_mixer"]
 
 
 class _Meta(type):
@@ -83,7 +83,7 @@ def _jsonable(v):
 def main():
     _install_stubs()
     sys.path.insert(0, str(REFERENCE))
-    # Only the five in-scope architecture modules are imported (the package __init__ would pull in
+    # Only the in-scope architecture modules are imported (the package __init__ would pull in
     # every family plus torch-based oracles).
     import importlib
 

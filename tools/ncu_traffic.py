@@ -25,6 +25,8 @@ FAMILIES = [
     # the TF32 instances of the wgmma GEMM (template argument A-transform = 2, fp32 out) before the bf16 ones
     ("gemm_wgmma_kernelILi64EfLi2E", "gemm_tf32"), ("gemm_wgmma_kernelILi128EfLi2E", "gemm_tf32"),
     ("gemm_wgmma", "gemm_bf16"), ("gemm_bf16_skinny", "gemm_bf16"),
+    # before "gemm_f32": the MLP-Mixer fp32 token-mixing kernel's name contains it
+    ("token_gemm_f32", "token_gemm_f32"), ("affine_kernel", "affine"),
     ("gemm_f32", "gemm_f32"),
     # before "attention_f32": the Segment Anything kernels' names contain it
     ("relpos_attention_bf16", "relpos_attention_bf16"), ("relpos_attention_f32", "relpos_attention_f32"),
