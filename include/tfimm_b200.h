@@ -76,7 +76,7 @@ int tfimm_b200_gemm_bf16_gated(const void* A, int lda, const float* gate, int ro
 /* Fused MLP block of the narrow stages:  out = residual + gamma * (act(A @ W1^T + b1) @ W2^T + b2).
  * A:[M,C] bf16 (the normalised activations), W1:[hidden,C] bf16, W2:[C,hidden] bf16, b1:[hidden], b2:[C], gamma:[C] or
  * NULL (ConvNeXt layer scale), residual / out:[M,C] fp32 (residual may alias out, or be NULL).  C in {96, 128, 192, 256},
- * hidden a multiple of 128: other shapes return TFIMM_B200_UNSUPPORTED and the caller runs two tfimm_b200_gemm_bf16.
+ * hidden a multiple of 128: other shapes return TFIMM_ERR_UNSUPPORTED and the caller runs two tfimm_b200_gemm_bf16.
  * One CTA per 128 rows walks the hidden dimension in chunks of 64: fc1 chunk (wgmma) -> bias + activation -> bf16
  * register fragments -> A operand of the fc2 chunk product (wgmma with A from registers); the [M,hidden]
  * activations never reach HBM (the hidden tensor is 61 % of the bytes the two-GEMM form moves at C = 128).  The
@@ -122,7 +122,7 @@ int tfimm_b200_conv_tf32(const float* x, const float* W, int ldw, const float* b
 
 /* ViT self-attention of tfimm_b200_attention_bf16 on fp32 qkv / out with TF32 products: q, k, v rounded to TF32
  * (cvt.rna) as they are loaded, fp32 online softmax, P rounded to TF32 before P V, fp32 accumulation.  K / V stream
- * through shared memory in 64-key blocks, so N is not limited.  dh == 64 (other head dims: TFIMM_B200_UNSUPPORTED). */
+ * through shared memory in 64-key blocks, so N is not limited.  dh == 64 (other head dims: TFIMM_ERR_UNSUPPORTED). */
 int tfimm_b200_attention_tf32(const float* qkv, float* out, int B, int N, int H, int dh, float scale, void* stream);
 
 /* LayerNorm over the last axis, fp32 statistics (tfimm/layers/factory.py:37-45).

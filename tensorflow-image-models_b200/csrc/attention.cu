@@ -203,9 +203,8 @@ int launch_vit_attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, in
     return kUnsupported;
   }
   auto kernel = vit_attention_bf16_kernel<NW, TPW>;
-  static unsigned long long attr_devs = 0;
-  if (first_use_on_device(attr_devs))
-    TFIMM_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  static std::atomic<unsigned long long> attr_devs{0};
+  TFIMM_CUDA_OK(set_max_dynamic_smem(kernel, 227 * 1024, attr_devs));
   dim3 grid((N + ROWS - 1) / ROWS, H, B);
   kernel<<<grid, NW * 32, smem, stream>>>(qkv, out, N, H, scale * 1.4426950408889634f);
   TFIMM_LAUNCH_OK("vit_attention_bf16_kernel");
@@ -433,8 +432,14 @@ __global__ void attention_f32_kernel(const float* __restrict__ qkv, float* __res
 
 }  // namespace
 
-int attention_bf16(const void* qkv, void* out, int B, int N, int H, int dh, float scale,
-                   cudaStream_t stream) {
+}  // namespace tfimm
+
+using namespace tfimm;
+
+extern "C" {
+
+int tfimm_b200_attention_bf16(const void* qkv, void* out, int B, int N, int H, int dh, float scale, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(B > 0 && N > 0 && H > 0, "attention: bad shape B=%d N=%d H=%d", B, N, H);
   if (dh != kDH) {
     set_last_error("attention: bf16 kernel supports head_dim 64 only (got %d)", dh);
@@ -450,7 +455,8 @@ int attention_bf16(const void* qkv, void* out, int B, int N, int H, int dh, floa
   return launch_vit_attention<7, 2>(q, o, B, N, H, scale, stream);
 }
 
-int attention_tf32(const float* qkv, float* out, int B, int N, int H, int dh, float scale, cudaStream_t stream) {
+int tfimm_b200_attention_tf32(const float* qkv, float* out, int B, int N, int H, int dh, float scale, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(B > 0 && N > 0 && H > 0, "attention_tf32: bad shape B=%d N=%d H=%d", B, N, H);
   if (dh != kDH) {
     set_last_error("attention_tf32: head_dim 64 only (got %d)", dh);
@@ -458,10 +464,8 @@ int attention_tf32(const float* qkv, float* out, int B, int N, int H, int dh, fl
   }
   TFIMM_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15u) == 0 && (reinterpret_cast<uintptr_t>(out) & 15u) == 0,
                   "attention_tf32: pointers must be 16-byte aligned");
-  static unsigned long long attr_devs = 0;
-  if (first_use_on_device(attr_devs))
-    TFIMM_CUDA_OK(cudaFuncSetAttribute(vit_attention_tf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)kTfSmemBytes));
+  static std::atomic<unsigned long long> attr_devs{0};
+  TFIMM_CUDA_OK(set_max_dynamic_smem(vit_attention_tf32_kernel, (int)kTfSmemBytes, attr_devs));
   dim3 grid((N + kTfRows - 1) / kTfRows, H, B);
   vit_attention_tf32_kernel<<<grid, kTfWarps * 32, kTfSmemBytes, stream>>>(qkv, out, N, H,
                                                                            scale * 1.4426950408889634f);
@@ -469,9 +473,9 @@ int attention_tf32(const float* qkv, float* out, int B, int N, int H, int dh, fl
   return kOk;
 }
 
-int attention_f32(const float* qkv, float* out, const float* bias, const float* mask, int nmask, long B,
-                  int N, int H, int dh, float scale, float* probs, const int* row_map, int nw_img,
-                  cudaStream_t stream) {
+int tfimm_b200_attention_f32(const float* qkv, float* out, const float* bias, const float* mask, int nmask, long B,
+                             int N, int H, int dh, float scale, float* probs, const int* row_map, int nw_img, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(row_map == nullptr || (nw_img > 0 && B % nw_img == 0), "attention_f32: bad window map");
   TFIMM_CHECK_ARG(B > 0 && N > 0 && H > 0 && dh > 0, "attention_f32: bad shape");
   const int warps = 4;
@@ -488,4 +492,4 @@ int attention_f32(const float* qkv, float* out, const float* bias, const float* 
   return kOk;
 }
 
-}  // namespace tfimm
+}  // extern "C"

@@ -81,8 +81,15 @@ attention_cls_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __res
 
 }  // namespace
 
-int attention_cls_bf16(const void* qkv, void* out, int B, int N, int H, int dh, int nq, float scale,
-                       cudaStream_t stream) {
+}  // namespace tfimm
+
+using namespace tfimm;
+
+extern "C" {
+
+int tfimm_b200_attention_cls_bf16(const void* qkv, void* out, int B, int N, int H, int dh, int nq, float scale,
+                                  void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(B > 0 && N > 0 && H > 0 && nq > 0 && nq <= N, "attention_cls: bad shape");
   TFIMM_CHECK_ARG(dh == kDh, "attention_cls: head_dim must be 64 (got %d)", dh);
   TFIMM_CHECK_ARG(N <= 32 * kMaxKeysPerLane, "attention_cls: at most %d tokens (got %d)", 32 * kMaxKeysPerLane, N);
@@ -93,4 +100,4 @@ int attention_cls_bf16(const void* qkv, void* out, int B, int N, int H, int dh, 
   return kOk;
 }
 
-}  // namespace tfimm
+}  // extern "C"

@@ -12,16 +12,20 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <atomic>
+
+#include "tfimm_b200.h"
+
 namespace tfimm {
 
 // ----------------------------------------------------------------------------
 // Status / error reporting (thread-local message, C ABI returns int status).
 // ----------------------------------------------------------------------------
 enum Status : int {
-  kOk = 0,
-  kInvalidArgument = 1,
-  kCudaError = 2,
-  kUnsupported = 3,
+  kOk = TFIMM_OK,
+  kInvalidArgument = TFIMM_ERR_INVALID_ARGUMENT,
+  kCudaError = TFIMM_ERR_CUDA,
+  kUnsupported = TFIMM_ERR_UNSUPPORTED,
 };
 
 void set_last_error(const char* fmt, ...);
@@ -47,31 +51,39 @@ int cuda_fail(cudaError_t e, const char* what);
     if (_e != cudaSuccess) return ::tfimm::cuda_fail(_e, name); \
   } while (0)
 
-// dtype codes shared with include/tfimm_b200.h
-enum DType : int { kF32 = 0, kBF16 = 1, kU8 = 2 };
+enum DType : int { kF32 = TFIMM_F32, kBF16 = TFIMM_BF16, kU8 = TFIMM_U8 };
 
-// activation codes shared with include/tfimm_b200.h
 enum Act : int {
-  kActNone = 0,
-  kActGelu = 1,    // exact erf form (Keras "gelu")
-  kActSwish = 2,   // x * sigmoid(x)
-  kActRelu = 3,
-  kActRelu6 = 4,
-  kActTanh = 5,
-  kActSigmoid = 6,
+  kActNone = TFIMM_ACT_NONE,
+  kActGelu = TFIMM_ACT_GELU,    // exact erf form (Keras "gelu")
+  kActSwish = TFIMM_ACT_SWISH,  // x * sigmoid(x)
+  kActRelu = TFIMM_ACT_RELU,
+  kActRelu6 = TFIMM_ACT_RELU6,
+  kActTanh = TFIMM_ACT_TANH,
+  kActSigmoid = TFIMM_ACT_SIGMOID,
 };
+
+// The C entry points take the stream as void* (the header is plain C).
+inline cudaStream_t as_stream(void* s) { return static_cast<cudaStream_t>(s); }
 
 int sm_count();  // of the CURRENT device (cached per device)
 
-// cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is a per-device setting: `mask` (one static per kernel
-// instantiation) remembers which devices have it.  Returns true the first time it is called for the current device.
-inline bool first_use_on_device(unsigned long long& mask) {
+// cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is a per-device setting: `devs` (one static per kernel
+// instantiation) records the devices it has been set on.  A device is recorded only once the call has succeeded, so no
+// thread launches before the attribute is in place, and a failed call is tried again on the next launch.
+// nonportable_cluster: also allow cluster sizes above 8 (cudaFuncAttributeNonPortableClusterSizeAllowed).
+template <typename Kernel>
+cudaError_t set_max_dynamic_smem(Kernel kernel, int bytes, std::atomic<unsigned long long>& devs,
+                                 bool nonportable_cluster = false) {
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev > 63) return true;
-  const unsigned long long bit = 1ull << dev;
-  if (mask & bit) return false;
-  mask |= bit;
-  return true;
+  const bool known = cudaGetDevice(&dev) == cudaSuccess && dev >= 0 && dev <= 63;
+  const unsigned long long bit = known ? 1ull << dev : 0;
+  if (known && (devs.load(std::memory_order_acquire) & bit)) return cudaSuccess;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e == cudaSuccess && nonportable_cluster)
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+  if (e == cudaSuccess) devs.fetch_or(bit, std::memory_order_release);
+  return e;
 }
 
 // tmap.cu: TMA descriptors (SWIZZLE_128B, zero OOB fill)

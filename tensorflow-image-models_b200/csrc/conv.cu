@@ -588,9 +588,29 @@ int im2col(const void* x, int in_dtype, void* out, int out_dtype, int B, int H, 
   return kOk;
 }
 
-int se_gate(const float* pooled_sum, float inv_hw, const float* w_reduce, const float* b_reduce,
-            const float* w_expand, const float* b_expand, float* gate, int B, int C, int rd, int act, int gate_act,
-            cudaStream_t stream) {
+}  // namespace tfimm
+
+using namespace tfimm;
+
+extern "C" {
+
+int tfimm_b200_im2col(const void* x, int in_dtype, void* out, int out_dtype, int B, int H, int W, int C, int groups,
+                      int ks, int stride, int pad_t, int pad_l, int Ho, int Wo, int Kpad, void* stream) {
+  return im2col(x, in_dtype, out, out_dtype, B, H, W, C, groups, ks, stride, pad_t, pad_l, Ho, Wo, Kpad,
+                as_stream(stream), 1.0f, nullptr, nullptr);
+}
+
+int tfimm_b200_im2col_u8(const void* x, void* out, int out_dtype, int B, int H, int W, int C, int ks, int stride,
+                         int pad_t, int pad_l, int Ho, int Wo, int Kpad, float scale, const float* mean,
+                         const float* inv_std, void* stream) {
+  return im2col(x, kU8, out, out_dtype, B, H, W, C, 1, ks, stride, pad_t, pad_l, Ho, Wo, Kpad, as_stream(stream), scale,
+                mean, inv_std);
+}
+
+int tfimm_b200_se_gate(const float* pooled_sum, float inv_hw, const float* w_reduce, const float* b_reduce,
+                       const float* w_expand, const float* b_expand, float* gate, int B, int C, int rd, int act,
+                       int gate_act, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(B > 0 && C > 0 && rd > 0, "se_gate: bad shape");
   const size_t smem = (size_t)(C + rd) * sizeof(float);
   TFIMM_CHECK_ARG(smem <= 48 * 1024, "se_gate: C + rd too large (%d + %d)", C, rd);
@@ -603,7 +623,8 @@ int se_gate(const float* pooled_sum, float inv_hw, const float* w_reduce, const 
   return kOk;
 }
 
-int scale_channels(void* x, int dtype, const float* gate, int B, int HW, int C, cudaStream_t stream) {
+int tfimm_b200_scale_channels(void* x, int dtype, const float* gate, int B, int HW, int C, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(B > 0 && HW > 0 && C > 0 && C % 8 == 0, "scale_channels: need C%%8==0 (C=%d)", C);
   const long total = (long)B * HW * (C / 8);
   const unsigned grid = conv_grid_for(total, 256);
@@ -619,8 +640,9 @@ int scale_channels(void* x, int dtype, const float* gate, int B, int HW, int C, 
   return kOk;
 }
 
-int pool2d(const void* x, int dtype, void* out, int B, int H, int W, int C, int ks, int stride, int pad_t,
-           int pad_l, int Ho, int Wo, int mode, cudaStream_t stream) {
+int tfimm_b200_pool2d(const void* x, int dtype, void* out, int B, int H, int W, int C, int ks, int stride, int pad_t,
+                      int pad_l, int Ho, int Wo, int mode, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(B > 0 && C % 8 == 0 && ks > 0 && stride > 0, "pool2d: need C%%8==0 (C=%d)", C);
   TFIMM_CHECK_ARG(mode >= 0 && mode <= 2, "pool2d: mode must be 0 (max), 1 (avg) or 2 (zero-padded max)");
   const long total = (long)B * Ho * Wo * (C / 8);
@@ -639,9 +661,10 @@ int pool2d(const void* x, int dtype, void* out, int B, int H, int W, int C, int 
   return kOk;
 }
 
-int dwconv_ln(const void* x, int in_dtype, const float* wgt, const float* bias, const float* gamma,
-              const float* beta, void* out, int out_dtype, int B, int H, int W, int C, int ks, float eps,
-              cudaStream_t stream) {
+int tfimm_b200_dwconv_ln(const void* x, int in_dtype, const float* wgt, const float* bias, const float* gamma,
+                         const float* beta, void* out, int out_dtype, int B, int H, int W, int C, int ks, float eps,
+                         void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(B > 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, "dwconv_ln: need C%%4==0 (C=%d)", C);
   TFIMM_CHECK_ARG(ks == 7, "dwconv_ln: only kernel size 7 is instantiated (got %d)", ks);
   {
@@ -688,9 +711,10 @@ int dwconv_ln(const void* x, int in_dtype, const float* wgt, const float* bias, 
   return kOk;
 }
 
-int dwconv_bias_act(const void* x, int dtype, const float* wgt, const float* bias, void* out, float* pool_sum,
-                    int B, int H, int W, int C, int ks, int stride, int pad_t, int pad_l, int Ho, int Wo,
-                    int act, cudaStream_t stream) {
+int tfimm_b200_dwconv_bias_act(const void* x, int dtype, const float* wgt, const float* bias, void* out,
+                               float* pool_sum, int B, int H, int W, int C, int ks, int stride, int pad_t, int pad_l,
+                               int Ho, int Wo, int act, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(B > 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, "dwconv: need C%%4==0 (C=%d)", C);
   TFIMM_CHECK_ARG((ks == 3 || ks == 5 || ks == 7) && (stride == 1 || stride == 2),
                   "dwconv: kernel size 3/5/7 and stride 1/2 are instantiated (got k=%d s=%d)", ks, stride);
@@ -734,7 +758,8 @@ int dwconv_bias_act(const void* x, int dtype, const float* wgt, const float* bia
   return kOk;
 }
 
-int global_avg_pool(const void* x, int dtype, float* out, int B, int HW, int C, cudaStream_t stream) {
+int tfimm_b200_global_avg_pool(const void* x, int dtype, float* out, int B, int HW, int C, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(B > 0 && HW > 0 && C > 0 && C % 4 == 0, "global_avg_pool: need C%%4==0");
   dim3 grid((C + 127) / 128, B);
   if (dtype == kBF16)
@@ -749,4 +774,4 @@ int global_avg_pool(const void* x, int dtype, float* out, int B, int HW, int C, 
   return kOk;
 }
 
-}  // namespace tfimm
+}  // extern "C"

@@ -117,8 +117,15 @@ inline unsigned grid_for(long total, int threads) {
 
 }  // namespace
 
-int patchify(const void* img, int in_dtype, void* out, int out_dtype, int B, int H, int W, int C, int p,
-             int Kpad, float scale, const float* mean, const float* inv_std, cudaStream_t stream) {
+}  // namespace tfimm
+
+using namespace tfimm;
+
+extern "C" {
+
+int tfimm_b200_patchify(const void* img, int in_dtype, void* out, int out_dtype, int B, int H, int W, int C, int p,
+                        int Kpad, float scale, const float* mean, const float* inv_std, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(B > 0 && p > 0 && H % p == 0 && W % p == 0, "patchify: H, W must be multiples of the patch size (H=%d W=%d p=%d)", H, W, p);
   TFIMM_CHECK_ARG(Kpad % 8 == 0 && Kpad >= p * p * C, "patchify: Kpad must be a multiple of 8 and >= p*p*C");
   TFIMM_CHECK_ARG((mean == nullptr) == (inv_std == nullptr), "patchify: mean and inv_std must be given together");
@@ -153,9 +160,9 @@ int patchify(const void* img, int in_dtype, void* out, int out_dtype, int B, int
   return kOk;
 }
 
-int assemble_tokens(const void* patches, int patch_dtype, const float* cls, const float* dist,
-                    const float* pos, void* out, int out_dtype, int B, int P, int ntok, int D,
-                    cudaStream_t stream) {
+int tfimm_b200_assemble_tokens(const void* patches, int patch_dtype, const float* cls, const float* dist,
+                               const float* pos, void* out, int out_dtype, int B, int P, int ntok, int D, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(B > 0 && P > 0 && D % 8 == 0 && (ntok == 1 || ntok == 2), "assemble_tokens: bad shape");
   TFIMM_CHECK_ARG(ntok == 1 || dist != nullptr, "assemble_tokens: dist token missing");
   const long total = (long)B * (P + ntok) * (D / 8);
@@ -177,7 +184,8 @@ int assemble_tokens(const void* patches, int patch_dtype, const float* cls, cons
   return kOk;
 }
 
-int cast_tensor(const void* in, int in_dtype, void* out, int out_dtype, long n, cudaStream_t stream) {
+int tfimm_b200_cast(const void* in, int in_dtype, void* out, int out_dtype, long n, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(n > 0, "cast: n must be positive");
   const int threads = 256;
   const unsigned grid = grid_for(n, threads);
@@ -197,4 +205,4 @@ int cast_tensor(const void* in, int in_dtype, void* out, int out_dtype, long n, 
   return kOk;
 }
 
-}  // namespace tfimm
+}  // extern "C"

@@ -159,10 +159,8 @@ int launch_dw_tma(const void* x, const float* wgt, const float* bias, void* out,
   int rc = make_tmap(&tmap, x, kBF16, 4, dims, strides, box, "dwconv input", /*swizzle_bytes=*/0);
   if (rc != kOk) return rc;
   auto kernel = dwconv_act_tma_kernel<KS, STRIDE, SHAPE>;
-  static unsigned long long attr_devs = 0;
-  if (first_use_on_device(attr_devs)) {
-    TFIMM_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-  }
+  static std::atomic<unsigned long long> attr_devs{0};
+  TFIMM_CUDA_OK(set_max_dynamic_smem(kernel, Cfg::kSmemBytes, attr_devs));
   const int tiles_x = (Wo + Cfg::TW - 1) / Cfg::TW, tiles_y = (Ho + Cfg::TH - 1) / Cfg::TH;
   const int cslabs = (C + kSlab - 1) / kSlab;
   const long grid = (long)B * tiles_y * tiles_x * cslabs;

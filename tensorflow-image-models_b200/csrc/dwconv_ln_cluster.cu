@@ -246,12 +246,9 @@ int launch_cluster(const void* x, const float* wgt, const float* bias, const flo
   using Cfg = DwCfg<CS>;
   auto kernel = dwconv7_ln_cluster_kernel<CS>;
   const int cl = C / CS;
-  static unsigned long long attr_devs = 0;
+  static std::atomic<unsigned long long> attr_devs{0};
   static int max_clusters[17] = {0};
-  if (first_use_on_device(attr_devs)) {
-    TFIMM_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    TFIMM_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-  }
+  TFIMM_CUDA_OK(set_max_dynamic_smem(kernel, Cfg::kSmemBytes, attr_devs, /*nonportable_cluster=*/true));
   const int tiles_x = (W + kTW - 1) / kTW, tiles_y = (H + kTH - 1) / kTH;
   const long n_tiles = (long)B * tiles_x * tiles_y;
 

@@ -64,9 +64,16 @@ gemm_f32_kernel(const float* __restrict__ A, int lda, const float* __restrict__ 
 
 }  // namespace
 
-int gemm_f32(const float* A, int lda, const float* W, int ldw, const float* bias, const float* gamma,
-             const float* residual, int ldr, float* C, int ldc, int M, int N, int K, int act, int act_post,
-             cudaStream_t stream) {
+}  // namespace tfimm
+
+using namespace tfimm;
+
+extern "C" {
+
+int tfimm_b200_gemm_f32(const float* A, int lda, const float* W, int ldw, const float* bias, const float* gamma,
+                        const float* residual, int ldr, float* C, int ldc, int M, int N, int K, int act, int act_post,
+                        void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(M > 0 && N > 0 && K > 0, "gemm_f32: M, N, K must be positive");
   TFIMM_CHECK_ARG(K % 4 == 0 && lda % 4 == 0 && ldw % 4 == 0, "gemm_f32: K, lda, ldw must be multiples of 4");
   TFIMM_CHECK_ARG((reinterpret_cast<uintptr_t>(A) & 15u) == 0 && (reinterpret_cast<uintptr_t>(W) & 15u) == 0,
@@ -77,4 +84,4 @@ int gemm_f32(const float* A, int lda, const float* W, int ldw, const float* bias
   return kOk;
 }
 
-}  // namespace tfimm
+}  // extern "C"

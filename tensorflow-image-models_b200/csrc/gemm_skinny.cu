@@ -175,10 +175,9 @@ int gemm_bf16_skinny(const void* A, int lda, const void* W, int ldw, const float
     return kUnsupported;
   const int n_rows_w = (N + 7) / 8 * 8;
   const int smem = n_rows_w * kSkRowBytes + 2 * kSkM * kSkRowBytes + n_rows_w * 4;
-  static unsigned long long attr_devs = 0;
-  if (first_use_on_device(attr_devs))
-    TFIMM_CUDA_OK(cudaFuncSetAttribute(gemm_bf16_skinny_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       kSkNMax * kSkRowBytes + 2 * kSkM * kSkRowBytes + kSkNMax * 4));
+  static std::atomic<unsigned long long> attr_devs{0};
+  TFIMM_CUDA_OK(set_max_dynamic_smem(gemm_bf16_skinny_kernel, kSkNMax * kSkRowBytes + 2 * kSkM * kSkRowBytes + kSkNMax * 4,
+                                     attr_devs));
   const int tiles = (M + kSkM - 1) / kSkM;
   const int per_sm = smem <= 56 * 1024 ? 3 : 2;   // co-resident CTAs (shared memory / 3 x 256 threads)
   const int max_ctas = per_sm * sm_count();

@@ -303,11 +303,39 @@ int check_out(const void* C, long ldc, const void* residual, long ldr, int esize
   return kOk;
 }
 
+// Every launch of a gemm_wgmma_kernel instance: the shared-memory attribute, one CTA per 128 x BLOCK_N output tile (per
+// image for token mixing), the launch and its error check.
+template <int BLOCK_N, typename OutT, int AX, int MODE>
+int launch_wgmma(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, const char* what,
+                 cudaStream_t stream) {
+  using Cfg = GemmCfg<BLOCK_N>;
+  auto kernel = gemm_wgmma_kernel<BLOCK_N, OutT, AX, MODE>;
+  static std::atomic<unsigned long long> attr_devs{0};  // per instantiation
+  TFIMM_CUDA_OK(set_max_dynamic_smem(kernel, Cfg::kSmemBytes, attr_devs));
+  const long imgs = MODE == kModeToken ? p.tk_imgs : 1;
+  const long tiles = imgs * ((p.M + kBlockM - 1) / kBlockM) * ((p.N + BLOCK_N - 1) / BLOCK_N);
+  kernel<<<(unsigned)tiles, gemm_threads<BLOCK_N, AX>(), Cfg::kSmemBytes, stream>>>(ta, tb, p);
+  TFIMM_LAUNCH_OK(what);
+  return kOk;
+}
+
+// Calls launch(std::integral_constant<int, BLOCK_N>{}) for the tile width bn.  kMaxN = 128 for the instances with
+// A-transform warps, which leave the consumers too few registers for a 256-wide accumulator.
+template <int kMaxN, typename F>
+int with_block_n(int bn, const char* unsupported_fmt, F&& launch) {
+  if constexpr (kMaxN >= 256) {
+    if (bn == 256) return launch(std::integral_constant<int, 256>{});
+  }
+  if (bn == 128) return launch(std::integral_constant<int, 128>{});
+  if (bn == 64) return launch(std::integral_constant<int, 64>{});
+  set_last_error(unsupported_fmt, bn);
+  return kInvalidArgument;
+}
+
 template <int BLOCK_N, typename OutT, int AX = kANone, int MODE = kModeGemm>
 int launch_gemm(const void* A, int lda, const void* W, int ldw, const void* residual, int ldr, void* C, int ldc,
                 GemmParams p, cudaStream_t stream) {
   const int M = p.M, N = p.N, K = p.K;
-  using Cfg = GemmCfg<BLOCK_N>;
   constexpr int kBlockK = block_k<AX>();
   CUtensorMap ta, tb;
   int st;
@@ -315,25 +343,17 @@ int launch_gemm(const void* A, int lda, const void* W, int ldw, const void* resi
   if ((st = make_tmap_2d(&ta, A, dtype_code<AX>(), M, K, lda, kBlockM, kBlockK, "A")) != kOk) return st;
   if ((st = make_tmap_2d(&tb, W, dtype_code<AX>(), N, K, ldw, BLOCK_N, kBlockK, "W")) != kOk) return st;
   p.c = C; p.res = residual; p.ldc = ldc; p.ldr = ldr;
-  auto kernel = gemm_wgmma_kernel<BLOCK_N, OutT, AX, MODE>;
-  static unsigned long long attr_devs = 0;  // per instantiation
-  if (first_use_on_device(attr_devs)) {
-    TFIMM_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-  }
-  const long tiles = (long)((M + kBlockM - 1) / kBlockM) * ((N + BLOCK_N - 1) / BLOCK_N);
-  kernel<<<(unsigned)tiles, gemm_threads<BLOCK_N, AX>(), Cfg::kSmemBytes, stream>>>(ta, tb, p);
-  TFIMM_LAUNCH_OK(AX == kATf32 ? "gemm_wgmma_kernel (tf32)"
-                               : (MODE == kModeGluCols ? "gemm_wgmma_kernel (bf16 glu)" : "gemm_wgmma_kernel (bf16)"));
-  return kOk;
+  return launch_wgmma<BLOCK_N, OutT, AX, MODE>(
+      ta, tb, p,
+      AX == kATf32 ? "gemm_wgmma_kernel (tf32)"
+                   : (MODE == kModeGluCols ? "gemm_wgmma_kernel (bf16 glu)" : "gemm_wgmma_kernel (bf16)"),
+      stream);
 }
-
-int pick_block_n(int M, int N);
 
 // Token mixing (kModeToken): A = Wt[M][K] (K-major, row stride ldw), B = X[imgs][K][N] (row stride ldx, image stride
 // img_x), both bf16.
 template <int BLOCK_N, typename OutT>
 int launch_token(const void* Wt, int ldw, const void* X, long ldx, long img_x, GemmParams p, cudaStream_t stream) {
-  using Cfg = GemmCfg<BLOCK_N>;
   CUtensorMap ta, tb;
   int st;
   if ((st = check_out(p.c, p.ldc, p.res, p.ldr, (int)sizeof(OutT))) != kOk) return st;
@@ -344,15 +364,7 @@ int launch_token(const void* Wt, int ldw, const void* X, long ldx, long img_x, G
     const uint32_t box[3] = {64u, 64u, 1u};
     if ((st = make_tmap(&tb, X, kBF16, 3, dims, strides, box, "token X")) != kOk) return st;
   }
-  auto kernel = gemm_wgmma_kernel<BLOCK_N, OutT, kANone, kModeToken>;
-  static unsigned long long attr_devs = 0;  // per instantiation
-  if (first_use_on_device(attr_devs)) {
-    TFIMM_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-  }
-  const long tiles = (long)p.tk_imgs * ((p.M + kBlockM - 1) / kBlockM) * ((p.N + BLOCK_N - 1) / BLOCK_N);
-  kernel<<<(unsigned)tiles, gemm_threads<BLOCK_N, kANone>(), Cfg::kSmemBytes, stream>>>(ta, tb, p);
-  TFIMM_LAUNCH_OK("gemm_wgmma_kernel (bf16 token mixing)");
-  return kOk;
+  return launch_wgmma<BLOCK_N, OutT, kANone, kModeToken>(ta, tb, p, "gemm_wgmma_kernel (bf16 token mixing)", stream);
 }
 
 // Implicit k x k convolution on the tensor cores: same kernel, A tensor map = the NHWC input (rank 4, traversal
@@ -360,7 +372,6 @@ int launch_token(const void* Wt, int ldw, const void* X, long ldx, long img_x, G
 template <int BLOCK_N, typename OutT, int AX = kANone>
 int launch_conv(const void* x, const void* W, int ldw, const void* residual, void* out, int B, int H, int Wd, int C,
                 int Ho, int Wo, GemmParams p, cudaStream_t stream) {
-  using Cfg = GemmCfg<BLOCK_N>;
   constexpr int kBlockK = block_k<AX>();
   constexpr uint64_t es = sizeof(OperandT<AX>);
   const int N = p.N, s = p.cv_stride;
@@ -377,16 +388,10 @@ int launch_conv(const void* x, const void* W, int ldw, const void* residual, voi
   if ((st = make_tmap_2d(&tb, W, dtype_code<AX>(), N, p.K, ldw, BLOCK_N, kBlockK, "conv weights")) != kOk) return st;
   p.c = out; p.res = residual; p.ldc = N; p.ldr = N;
   p.cv_B = B; p.cv_Ho = Ho; p.cv_Wo = Wo;
-  auto kernel = gemm_wgmma_kernel<BLOCK_N, OutT, AX>;
-  static unsigned long long attr_devs = 0;  // per instantiation
-  if (first_use_on_device(attr_devs)) {
-    TFIMM_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-  }
-  const long tiles = (long)(p.M / kBlockM) * ((N + BLOCK_N - 1) / BLOCK_N);
-  kernel<<<(unsigned)tiles, gemm_threads<BLOCK_N, AX>(), Cfg::kSmemBytes, stream>>>(ta, tb, p);
-  TFIMM_LAUNCH_OK(AX == kATf32 ? "gemm_wgmma_kernel (tf32 implicit convolution)"
-                                  : "gemm_wgmma_kernel (bf16 implicit convolution)");
-  return kOk;
+  return launch_wgmma<BLOCK_N, OutT, AX, kModeGemm>(
+      ta, tb, p,
+      AX == kATf32 ? "gemm_wgmma_kernel (tf32 implicit convolution)" : "gemm_wgmma_kernel (bf16 implicit convolution)",
+      stream);
 }
 
 int pick_block_n(int M, int N) {
@@ -413,65 +418,6 @@ int pick_block_n(int M, int N) {
 int gemm_bf16_skinny(const void* A, int lda, const void* W, int ldw, const float* bias, const void* residual, int ldr,
                      void* C, int ldc, int M, int N, int K, int act, cudaStream_t stream, const float* gate = nullptr,
                      int rows_per_img = 1, int imgs = 1);
-
-int gemm_bf16_dispatch(const void* A, int lda, const void* W, int ldw, const float* bias,
-                       const float* gamma, const void* residual, int ldr, void* C, int ldc, int M,
-                       int N, int K, int act, int act_post, int out_dtype, int force_block_n, cudaStream_t stream) {
-  TFIMM_CHECK_ARG(M > 0 && N > 0 && K > 0, "gemm: M, N, K must be positive (got %d %d %d)", M, N, K);
-  TFIMM_CHECK_ARG(out_dtype == kBF16 || out_dtype == kF32, "gemm: out_dtype must be bf16 or f32");
-  TFIMM_CHECK_ARG(K % 8 == 0, "gemm: K must be a multiple of 8 (got %d)", K);
-  TFIMM_CHECK_ARG(bias == nullptr || (reinterpret_cast<uintptr_t>(bias) & 15u) == 0, "gemm: bias must be 16-byte aligned");
-  TFIMM_CHECK_ARG(gamma == nullptr || (reinterpret_cast<uintptr_t>(gamma) & 15u) == 0, "gemm: gamma must be 16-byte aligned");
-  if (force_block_n == 0 && K <= 64 && out_dtype == kBF16 && gamma == nullptr && act_post == 0) {
-    // short contraction: streaming mma.sync kernel (gemm_skinny.cu); kUnsupported = shape outside its envelope
-    const int st = gemm_bf16_skinny(A, lda, W, ldw, bias, residual, ldr, C, ldc, M, N, K, act, stream);
-    if (st != kUnsupported) return st;
-  }
-  GemmParams p{};
-  p.M = M; p.N = N; p.K = K;
-  p.bias = bias; p.gamma = gamma; p.act = act; p.has_res = residual != nullptr ? 1 : 0; p.act_post = act_post;
-  // force_block_n: 0 = choose; 64/128/256 = that tile width; 2 = the widest tile (256)
-  const int bn = force_block_n == 2 ? 256 : (force_block_n > 0 ? force_block_n : pick_block_n(M, N));
-#define TFIMM_GEMM_CASE(BN)                                                                         \
-  case BN:                                                                                          \
-    return out_dtype == kBF16 ? launch_gemm<BN, __nv_bfloat16>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream) \
-                              : launch_gemm<BN, float>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream);
-  switch (bn) {
-    TFIMM_GEMM_CASE(256)
-    TFIMM_GEMM_CASE(128)
-    TFIMM_GEMM_CASE(64)
-    default:
-      set_last_error("gemm: unsupported block_n %d", bn);
-      return kInvalidArgument;
-  }
-#undef TFIMM_GEMM_CASE
-}
-
-// Dense layer whose input rows are first multiplied by a per-image channel gate (squeeze-excite): the projection
-// convolutions after SEModule (tfimm/layers/attention.py, efficientnet_blocks.py:241-248, 438-453).  bf16 out.
-int gemm_bf16_gated_dispatch(const void* A, int lda, const float* gate, int rows_per_img, int imgs, const void* W, int ldw,
-                             const float* bias, const void* residual, int ldr, void* C, int ldc, int M, int N, int K,
-                             int act, cudaStream_t stream) {
-  TFIMM_CHECK_ARG(M > 0 && N > 0 && K > 0 && K % 8 == 0, "gemm_gated: need K %% 8 == 0 (got M=%d N=%d K=%d)", M, N, K);
-  TFIMM_CHECK_ARG(gate != nullptr && rows_per_img > 0 && imgs > 0 && (reinterpret_cast<uintptr_t>(gate) & 15u) == 0,
-                  "gemm_gated: gate [imgs][K] fp32, 16-byte aligned");
-  TFIMM_CHECK_ARG(bias == nullptr || (reinterpret_cast<uintptr_t>(bias) & 15u) == 0, "gemm_gated: bias must be 16-byte aligned");
-  if (K <= 64) {   // short contraction: the streaming kernel scales its A fragments in registers
-    const int st = gemm_bf16_skinny(A, lda, W, ldw, bias, residual, ldr, C, ldc, M, N, K, act, stream, gate, rows_per_img,
-                                    imgs);
-    if (st != kUnsupported) return st;
-  }
-  GemmParams p{};
-  p.M = M; p.N = N; p.K = K;
-  p.bias = bias; p.act = act; p.has_res = residual != nullptr ? 1 : 0;
-  p.a_scale = gate; p.a_rows_per_img = rows_per_img; p.a_imgs = imgs;
-  // at most 128 columns: the gate warps leave the consumers too few registers for a 256-wide accumulator
-  switch (pick_block_n(M, N)) {
-    case 256:
-    case 128: return launch_gemm<128, __nv_bfloat16, kAGate>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream);
-    default: return launch_gemm<64, __nv_bfloat16, kAGate>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream);
-  }
-}
 
 // k x k convolution (stride 1 or 2, symmetric padding (k-1)/2... given as `pad`) + bias + activation (+ residual),
 // NHWC bf16 in, NHWC bf16/fp32 out, W[N][k*k*C] in (ky, kx, c) order: implicit GEMM, no im2col matrix in HBM.
@@ -500,36 +446,86 @@ int conv_setup(GemmParams& p, const float* bias, const void* residual, int B, in
   return kOk;
 }
 
-int conv_bf16_dispatch(const void* x, const void* W, int ldw, const float* bias, const void* residual, void* out,
-                       int B, int H, int Wd, int C, int N, int ks, int stride, int pad, int act, int act_post,
-                       int out_dtype, cudaStream_t stream) {
+}  // namespace tfimm
+
+using namespace tfimm;
+
+extern "C" {
+
+int tfimm_b200_gemm_bf16(const void* A, int lda, const void* W, int ldw, const float* bias, const float* gamma,
+                         const void* residual, int ldr, void* C, int ldc, int M, int N, int K, int act, int act_post,
+                         int out_dtype, int force_block_n, void* s) {
+  const cudaStream_t stream = as_stream(s);
+  TFIMM_CHECK_ARG(M > 0 && N > 0 && K > 0, "gemm: M, N, K must be positive (got %d %d %d)", M, N, K);
+  TFIMM_CHECK_ARG(out_dtype == kBF16 || out_dtype == kF32, "gemm: out_dtype must be bf16 or f32");
+  TFIMM_CHECK_ARG(K % 8 == 0, "gemm: K must be a multiple of 8 (got %d)", K);
+  TFIMM_CHECK_ARG(bias == nullptr || (reinterpret_cast<uintptr_t>(bias) & 15u) == 0, "gemm: bias must be 16-byte aligned");
+  TFIMM_CHECK_ARG(gamma == nullptr || (reinterpret_cast<uintptr_t>(gamma) & 15u) == 0, "gemm: gamma must be 16-byte aligned");
+  if (force_block_n == 0 && K <= 64 && out_dtype == kBF16 && gamma == nullptr && act_post == 0) {
+    // short contraction: streaming mma.sync kernel (gemm_skinny.cu); kUnsupported = shape outside its envelope
+    const int st = gemm_bf16_skinny(A, lda, W, ldw, bias, residual, ldr, C, ldc, M, N, K, act, stream);
+    if (st != kUnsupported) return st;
+  }
+  GemmParams p{};
+  p.M = M; p.N = N; p.K = K;
+  p.bias = bias; p.gamma = gamma; p.act = act; p.has_res = residual != nullptr ? 1 : 0; p.act_post = act_post;
+  // force_block_n: 0 = choose; 64/128/256 = that tile width; 2 = the widest tile (256)
+  const int bn = force_block_n == 2 ? 256 : (force_block_n > 0 ? force_block_n : pick_block_n(M, N));
+  return with_block_n<256>(bn, "gemm: unsupported block_n %d", [&](auto n) {
+    constexpr int BN = decltype(n)::value;
+    return out_dtype == kBF16 ? launch_gemm<BN, __nv_bfloat16>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream)
+                              : launch_gemm<BN, float>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream);
+  });
+}
+
+// Dense layer whose input rows are first multiplied by a per-image channel gate (squeeze-excite): the projection
+// convolutions after SEModule (tfimm/layers/attention.py, efficientnet_blocks.py:241-248, 438-453).  bf16 out.
+int tfimm_b200_gemm_bf16_gated(const void* A, int lda, const float* gate, int rows_per_img, int imgs, const void* W,
+                               int ldw, const float* bias, const void* residual, int ldr, void* C, int ldc, int M,
+                               int N, int K, int act, void* s) {
+  const cudaStream_t stream = as_stream(s);
+  TFIMM_CHECK_ARG(M > 0 && N > 0 && K > 0 && K % 8 == 0, "gemm_gated: need K %% 8 == 0 (got M=%d N=%d K=%d)", M, N, K);
+  TFIMM_CHECK_ARG(gate != nullptr && rows_per_img > 0 && imgs > 0 && (reinterpret_cast<uintptr_t>(gate) & 15u) == 0,
+                  "gemm_gated: gate [imgs][K] fp32, 16-byte aligned");
+  TFIMM_CHECK_ARG(bias == nullptr || (reinterpret_cast<uintptr_t>(bias) & 15u) == 0, "gemm_gated: bias must be 16-byte aligned");
+  if (K <= 64) {   // short contraction: the streaming kernel scales its A fragments in registers
+    const int st = gemm_bf16_skinny(A, lda, W, ldw, bias, residual, ldr, C, ldc, M, N, K, act, stream, gate, rows_per_img,
+                                    imgs);
+    if (st != kUnsupported) return st;
+  }
+  GemmParams p{};
+  p.M = M; p.N = N; p.K = K;
+  p.bias = bias; p.act = act; p.has_res = residual != nullptr ? 1 : 0;
+  p.a_scale = gate; p.a_rows_per_img = rows_per_img; p.a_imgs = imgs;
+  return with_block_n<128>(pick_block_n(M, N) == 64 ? 64 : 128, "gemm_gated: unsupported block_n %d", [&](auto n) {
+    return launch_gemm<decltype(n)::value, __nv_bfloat16, kAGate>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream);
+  });
+}
+
+int tfimm_b200_conv_bf16(const void* x, const void* W, int ldw, const float* bias, const void* residual, void* out,
+                         int B, int H, int Wd, int C, int N, int ks, int stride, int pad, int act, int act_post,
+                         int out_dtype, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(out_dtype == kBF16 || out_dtype == kF32, "conv: out_dtype must be bf16 or f32");
   GemmParams p;
   int Ho, Wo, st;
   if ((st = conv_setup(p, bias, residual, B, H, Wd, C, N, ks, stride, pad, act, act_post, 64, Ho, Wo)) != kOk)
     return st;
-  const int bn = N >= 256 ? 256 : (N >= 128 ? 128 : 64);
-#define TFIMM_CONV_CASE(BN)                                                                                       \
-  case BN:                                                                                                        \
-    return out_dtype == kBF16                                                                                     \
-               ? launch_conv<BN, __nv_bfloat16>(x, W, ldw, residual, out, B, H, Wd, C, Ho, Wo, p, stream)           \
-               : launch_conv<BN, float>(x, W, ldw, residual, out, B, H, Wd, C, Ho, Wo, p, stream);
-  switch (bn) {
-    TFIMM_CONV_CASE(256)
-    TFIMM_CONV_CASE(128)
-    TFIMM_CONV_CASE(64)
-  }
-#undef TFIMM_CONV_CASE
-  return kInvalidArgument;
+  return with_block_n<256>(N >= 256 ? 256 : (N >= 128 ? 128 : 64), "conv: unsupported block_n %d", [&](auto n) {
+    constexpr int BN = decltype(n)::value;
+    return out_dtype == kBF16 ? launch_conv<BN, __nv_bfloat16>(x, W, ldw, residual, out, B, H, Wd, C, Ho, Wo, p, stream)
+                              : launch_conv<BN, float>(x, W, ldw, residual, out, B, H, Wd, C, Ho, Wo, p, stream);
+  });
 }
 
 // ---- precision="tf32": fp32 operands, TF32 tensor-core products, fp32 out ----
 // W must already be TF32-representable (low 13 bits zero: rounded once at plan time); the A tiles are rounded in shared
 // memory by the transform warps.  At most 128 columns: the transform warps leave the consumers too few registers for a
 // 256-wide accumulator (as in the gated instances).
-int gemm_tf32_dispatch(const float* A, int lda, const float* W, int ldw, const float* bias, const float* gamma,
-                       const float* residual, int ldr, float* C, int ldc, int M, int N, int K, int act, int act_post,
-                       int force_block_n, cudaStream_t stream) {
+int tfimm_b200_gemm_tf32(const float* A, int lda, const float* W, int ldw, const float* bias, const float* gamma,
+                         const float* residual, int ldr, float* C, int ldc, int M, int N, int K, int act, int act_post,
+                         int force_block_n, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(M > 0 && N > 0 && K > 0, "gemm_tf32: M, N, K must be positive (got %d %d %d)", M, N, K);
   TFIMM_CHECK_ARG(K % 4 == 0, "gemm_tf32: K must be a multiple of 4 (got %d)", K);
   TFIMM_CHECK_ARG(bias == nullptr || (reinterpret_cast<uintptr_t>(bias) & 15u) == 0, "gemm_tf32: bias must be 16-byte aligned");
@@ -540,36 +536,35 @@ int gemm_tf32_dispatch(const float* A, int lda, const float* W, int ldw, const f
   p.bias = bias; p.gamma = gamma; p.act = act; p.has_res = residual != nullptr ? 1 : 0; p.act_post = act_post;
   // force_block_n: 0 = choose; 64 / 128 = that tile width; 2 = the widest tile (128)
   const int bn = force_block_n == 2 ? 128 : (force_block_n > 0 ? force_block_n : (pick_block_n(M, N) == 64 ? 64 : 128));
-  switch (bn) {
-    case 128: return launch_gemm<128, float, kATf32>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream);
-    case 64: return launch_gemm<64, float, kATf32>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream);
-    default:
-      set_last_error("gemm_tf32: unsupported block_n %d (64 or 128)", bn);
-      return kInvalidArgument;
-  }
+  return with_block_n<128>(bn, "gemm_tf32: unsupported block_n %d (64 or 128)", [&](auto n) {
+    return launch_gemm<decltype(n)::value, float, kATf32>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream);
+  });
 }
 
-// k x k convolution as conv_bf16_dispatch, fp32 NHWC in / out with TF32 products; C % 32 == 0 (one 32-channel fp32 box
+// k x k convolution as tfimm_b200_conv_bf16, fp32 NHWC in / out with TF32 products; C % 32 == 0 (one 32-channel fp32 box
 // per k-block).
-int conv_tf32_dispatch(const float* x, const float* W, int ldw, const float* bias, const float* residual, float* out,
-                       int B, int H, int Wd, int C, int N, int ks, int stride, int pad, int act, int act_post,
-                       cudaStream_t stream) {
+int tfimm_b200_conv_tf32(const float* x, const float* W, int ldw, const float* bias, const float* residual, float* out,
+                         int B, int H, int Wd, int C, int N, int ks, int stride, int pad, int act, int act_post,
+                         void* s) {
+  const cudaStream_t stream = as_stream(s);
   GemmParams p;
   int Ho, Wo, st;
   if ((st = conv_setup(p, bias, residual, B, H, Wd, C, N, ks, stride, pad, act, act_post, 32, Ho, Wo)) != kOk)
     return st;
-  if (N >= 128) return launch_conv<128, float, kATf32>(x, W, ldw, residual, out, B, H, Wd, C, Ho, Wo, p, stream);
-  return launch_conv<64, float, kATf32>(x, W, ldw, residual, out, B, H, Wd, C, Ho, Wo, p, stream);
+  return with_block_n<128>(N >= 128 ? 128 : 64, "conv: unsupported block_n %d", [&](auto n) {
+    return launch_conv<decltype(n)::value, float, kATf32>(x, W, ldw, residual, out, B, H, Wd, C, Ho, Wo, p, stream);
+  });
 }
 
 // ---- MLP-Mixer family (tfimm.backend.mixer_ops) ----
 // Token mixing: out[b][m][c] = epi(sum_n Wt[m][n] X[b][n][c]), see GemmParams (kModeToken) for the epilogue.
 // Wt: bf16 [M][K], row stride ldw % 8 == 0 (rows padded at plan time); X: bf16, row stride ldx and image stride img_x,
 // both multiples of 8 elements.  out / residual / mul: bf16 or fp32 (out_dtype), rows of N elements.
-int token_gemm_bf16_dispatch(const void* Wt, int ldw, const void* X, long ldx, long img_x, const float* bias,
-                             const float* gamma, const void* residual, long ldr, long img_r, const void* mul, long ld_mul,
-                             long img_mul, void* out, long ldc, long img_c, int imgs, int M, int N, int K, int m_out,
-                             int act, int glu, int out_dtype, int force_block_n, cudaStream_t stream) {
+int tfimm_b200_token_gemm_bf16(const void* Wt, int ldw, const void* X, long ldx, long img_x, const float* bias,
+                               const float* gamma, const void* residual, long ldr, long img_r, const void* mul,
+                               long ld_mul, long img_mul, void* out, long ldc, long img_c, int imgs, int M, int N,
+                               int K, int m_out, int act, int glu, int out_dtype, int force_block_n, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(imgs > 0 && M > 0 && N > 0 && K > 0 && m_out > 0, "token_gemm: empty shape (imgs %d M %d N %d K %d)",
                   imgs, M, N, K);
   TFIMM_CHECK_ARG(out_dtype == kBF16 || out_dtype == kF32, "token_gemm: out_dtype must be bf16 or f32");
@@ -592,26 +587,19 @@ int token_gemm_bf16_dispatch(const void* Wt, int ldw, const void* X, long ldx, l
   p.tk_imgs = imgs; p.m_out = m_out; p.glu = glu; p.img_c = img_c; p.img_r = img_r;
   p.mul = mul; p.ld_mul = ld_mul; p.img_mul = img_mul;
   const int bn = force_block_n > 0 ? force_block_n : pick_block_n(imgs * ((M + kBlockM - 1) / kBlockM) * kBlockM, N);
-#define TFIMM_TOKEN_CASE(BN)                                                                              \
-  case BN:                                                                                                \
-    return out_dtype == kBF16 ? launch_token<BN, __nv_bfloat16>(Wt, ldw, X, ldx, img_x, p, stream)       \
+  return with_block_n<256>(bn, "token_gemm: unsupported block_n %d", [&](auto n) {
+    constexpr int BN = decltype(n)::value;
+    return out_dtype == kBF16 ? launch_token<BN, __nv_bfloat16>(Wt, ldw, X, ldx, img_x, p, stream)
                               : launch_token<BN, float>(Wt, ldw, X, ldx, img_x, p, stream);
-  switch (bn) {
-    TFIMM_TOKEN_CASE(256)
-    TFIMM_TOKEN_CASE(128)
-    TFIMM_TOKEN_CASE(64)
-    default:
-      set_last_error("token_gemm: unsupported block_n %d", bn);
-      return kInvalidArgument;
-  }
-#undef TFIMM_TOKEN_CASE
+  });
 }
 
 // Channel GLU (gMixer's mlp_channels fc1): W rows 2j / 2j + 1 are value / gate feature j (interleaved at plan time),
 // bias likewise; out[M][N / 2] = (A W_value^T + b) * act(A W_gate^T + b), bf16.  The full-width hidden tensor is never
 // written.
-int gemm_glu_bf16_dispatch(const void* A, int lda, const void* W, int ldw, const float* bias, void* C, int ldc, int M,
-                           int N, int K, int act, int force_block_n, cudaStream_t stream) {
+int tfimm_b200_gemm_glu_bf16(const void* A, int lda, const void* W, int ldw, const float* bias, void* C, int ldc, int M,
+                             int N, int K, int act, int force_block_n, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(M > 0 && N > 0 && K > 0 && K % 8 == 0 && N % 2 == 0,
                   "gemm_glu: need K %% 8 == 0 and an even N (got M=%d N=%d K=%d)", M, N, K);
   TFIMM_CHECK_ARG(bias == nullptr || (reinterpret_cast<uintptr_t>(bias) & 7u) == 0, "gemm_glu: bias must be 8-byte aligned");
@@ -619,14 +607,10 @@ int gemm_glu_bf16_dispatch(const void* A, int lda, const void* W, int ldw, const
   p.M = M; p.N = N; p.K = K;
   p.bias = bias; p.act = act;
   const int bn = force_block_n > 0 ? force_block_n : pick_block_n(M, N);
-  switch (bn) {
-    case 256: return launch_gemm<256, __nv_bfloat16, kANone, kModeGluCols>(A, lda, W, ldw, nullptr, 0, C, ldc, p, stream);
-    case 128: return launch_gemm<128, __nv_bfloat16, kANone, kModeGluCols>(A, lda, W, ldw, nullptr, 0, C, ldc, p, stream);
-    case 64: return launch_gemm<64, __nv_bfloat16, kANone, kModeGluCols>(A, lda, W, ldw, nullptr, 0, C, ldc, p, stream);
-    default:
-      set_last_error("gemm_glu: unsupported block_n %d", bn);
-      return kInvalidArgument;
-  }
+  return with_block_n<256>(bn, "gemm_glu: unsupported block_n %d", [&](auto n) {
+    return launch_gemm<decltype(n)::value, __nv_bfloat16, kANone, kModeGluCols>(A, lda, W, ldw, nullptr, 0, C, ldc, p,
+                                                                               stream);
+  });
 }
 
-}  // namespace tfimm
+}  // extern "C"

@@ -97,11 +97,18 @@ __global__ void affine_kernel(const float* __restrict__ x, long ldx, const float
 
 }  // namespace
 
-// Token mixing in fp32 (precision="fp32"): the contract of token_gemm_bf16_dispatch with fp32 operands and output.
-int token_gemm_f32(const float* Wt, int ldw, const float* X, long ldx, long img_x, const float* bias, const float* gamma,
-                   const float* residual, long ldr, long img_r, const float* mul, long ld_mul, long img_mul, float* out,
-                   long ldc, long img_c, int imgs, int M, int N, int K, int m_out, int act, int glu,
-                   cudaStream_t stream) {
+}  // namespace tfimm
+
+using namespace tfimm;
+
+extern "C" {
+
+// Token mixing in fp32 (precision="fp32"): the contract of tfimm_b200_token_gemm_bf16 with fp32 operands and output.
+int tfimm_b200_token_gemm_f32(const float* Wt, int ldw, const float* X, long ldx, long img_x, const float* bias,
+                              const float* gamma, const float* residual, long ldr, long img_r, const float* mul,
+                              long ld_mul, long img_mul, float* out, long ldc, long img_c, int imgs, int M, int N,
+                              int K, int m_out, int act, int glu, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(imgs > 0 && M > 0 && N > 0 && K > 0 && m_out > 0 && ldw >= K,
                   "token_gemm_f32: bad shape (imgs %d M %d N %d K %d)", imgs, M, N, K);
   TFIMM_CHECK_ARG(glu ? (M % 16 == 0 && m_out <= M / 2) : m_out <= M, "token_gemm_f32: m_out %d does not fit M %d",
@@ -116,8 +123,9 @@ int token_gemm_f32(const float* Wt, int ldw, const float* X, long ldx, long img_
 
 // Channel GLU in fp32: out[M][n_out] = (A W_value^T + b) * act(A W_gate^T + b) with W's rows in the SIMT kernel's
 // pairing (per 16 rows: 8 value features, then their 8 gates), run as a token GEMM whose "tokens" are A's columns.
-int gemm_glu_f32(const float* A, int lda, const float* W, int ldw, const float* bias, float* C, int ldc, int M, int N,
-                 int n_out, int K, int act, cudaStream_t stream) {
+int tfimm_b200_gemm_glu_f32(const float* A, int lda, const float* W, int ldw, const float* bias, float* C, int ldc,
+                            int M, int N, int n_out, int K, int act, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(M > 0 && N > 0 && K > 0 && N % 16 == 0 && ldw >= K && n_out > 0 && n_out <= N / 2,
                   "gemm_glu_f32: need N %% 16 == 0 and n_out <= N / 2 (got N %d, n_out %d)", N, n_out);
   TokenF32Params p{W, ldw, A, 0, 1, lda, bias, nullptr, nullptr, 0, 0, nullptr, 0, 0,
@@ -128,8 +136,9 @@ int gemm_glu_f32(const float* A, int lda, const float* W, int ldw, const float* 
   return kOk;
 }
 
-int affine(const float* x, long ldx, const float* alpha, const float* beta, void* out, int out_dtype, long ldo,
-           long rows, int C, cudaStream_t stream) {
+int tfimm_b200_affine(const float* x, long ldx, const float* alpha, const float* beta, void* out, int out_dtype,
+                      long ldo, long rows, int C, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(rows > 0 && C > 0 && ldx >= C && ldo >= C, "affine: bad shape");
   TFIMM_CHECK_ARG(out_dtype == kBF16 || out_dtype == kF32, "affine: out_dtype must be bf16 or f32");
   const long n = rows * C;
@@ -142,4 +151,4 @@ int affine(const float* x, long ldx, const float* alpha, const float* beta, void
   return kOk;
 }
 
-}  // namespace tfimm
+}  // extern "C"

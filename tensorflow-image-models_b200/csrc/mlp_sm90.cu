@@ -154,9 +154,8 @@ int launch_mlp(const void* A, int lda, const void* W1, int ldw1, const float* b1
   if ((st = make_tmap_2d(&tw1, W1, kBF16, hidden, C, ldw1, kHC, 64, "W1")) != kOk) return st;
   if ((st = make_tmap_2d(&tw2, W2, kBF16, C, hidden, ldw2, C, 64, "W2")) != kOk) return st;
   auto kernel = mlp_fused_wgmma_kernel<C>;
-  static unsigned long long attr_devs = 0;
-  if (first_use_on_device(attr_devs))
-    TFIMM_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+  static std::atomic<unsigned long long> attr_devs{0};
+  TFIMM_CUDA_OK(set_max_dynamic_smem(kernel, Cfg::kSmemBytes, attr_devs));
   const int tiles = (p.M + kMlpRows - 1) / kMlpRows;
   kernel<<<tiles, kMlpThreads, Cfg::kSmemBytes, stream>>>(ta, tw1, tw2, b1, hidden, act, p);
   TFIMM_LAUNCH_OK("mlp_fused_wgmma_kernel");
@@ -165,10 +164,17 @@ int launch_mlp(const void* A, int lda, const void* W1, int ldw1, const float* b1
 
 }  // namespace
 
+}  // namespace tfimm
+
+using namespace tfimm;
+
+extern "C" {
+
 // Returns kUnsupported for shapes outside the kernel (the caller then runs the two GEMMs).
-int mlp_fused_bf16(const void* A, int lda, const void* W1, int ldw1, const float* b1, const void* W2, int ldw2,
-                   const float* b2, const float* gamma, const void* residual, int ldr, void* out, int ldc, int M, int C,
-                   int H, int act, cudaStream_t stream) {
+int tfimm_b200_mlp_bf16(const void* A, int lda, const void* W1, int ldw1, const float* b1, const void* W2, int ldw2,
+                        const float* b2, const float* gamma, const void* residual, int ldr, void* out, int ldc, int M,
+                        int C, int H, int act, void* s) {
+  const cudaStream_t stream = as_stream(s);
   if ((C != 96 && C != 128 && C != 192 && C != 256) || H % 128 != 0 || H < 256 || M < 1) {
     set_last_error("mlp_fused: needs C in {96, 128, 192, 256} and hidden %% 128 == 0, >= 256 (got C=%d hidden=%d)", C, H);
     return kUnsupported;
@@ -197,4 +203,4 @@ int mlp_fused_bf16(const void* A, int lda, const void* W1, int ldw1, const float
   }
 }
 
-}  // namespace tfimm
+}  // extern "C"

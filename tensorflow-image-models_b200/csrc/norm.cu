@@ -257,12 +257,17 @@ int dispatch_ln(int in_dtype, int out_dtype, const float* gamma, const float* be
   return kInvalidArgument;
 }
 
-
 }  // namespace
 
-int layernorm_rows(const void* x, int in_dtype, long in_stride, const float* gamma, const float* beta,
-                   void* out, int out_dtype, long out_stride, long rows, int C, float eps,
-                   cudaStream_t stream) {
+}  // namespace tfimm
+
+using namespace tfimm;
+
+extern "C" {
+
+int tfimm_b200_layernorm(const void* x, int in_dtype, long in_stride, const float* gamma, const float* beta, void* out,
+                         int out_dtype, long out_stride, long rows, int C, float eps, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(rows > 0 && C > 0 && C % 8 == 0, "layernorm: need rows>0 and C%%8==0 (rows=%ld C=%d)", rows, C);
   TFIMM_CHECK_ARG(in_stride % 8 == 0 && out_stride % 8 == 0, "layernorm: strides must be multiples of 8 elements");
   if (in_dtype == kF32 && C % 4 == 0 && in_stride % 4 == 0 && out_stride % 4 == 0 &&
@@ -279,20 +284,22 @@ int layernorm_rows(const void* x, int in_dtype, long in_stride, const float* gam
   return dispatch_ln(in_dtype, out_dtype, gamma, beta, rows, C, eps, map, stream);
 }
 
-int layernorm_patch2x2(const void* x, int in_dtype, const float* gamma, const float* beta, void* out,
-                       int out_dtype, int B, int H, int W, int C, float eps, cudaStream_t stream) {
+int tfimm_b200_layernorm_patch2x2(const void* x, int in_dtype, const float* gamma, const float* beta, void* out,
+                                  int out_dtype, int B, int H, int W, int C, float eps, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(B > 0 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0 && C % 8 == 0,
                   "layernorm_patch2x2: need even H, W and C%%8==0 (H=%d W=%d C=%d)", H, W, C);
   Patch2x2Rows map{x, out, H, W, C};
   return dispatch_ln(in_dtype, out_dtype, gamma, beta, (long)B * H * W, C, eps, map, stream);
 }
 
-int patch_merge_ln(const void* x, int in_dtype, const float* gamma, const float* beta, void* out,
-                   int out_dtype, int B, int H, int W, int C, float eps, cudaStream_t stream) {
+int tfimm_b200_patch_merge_ln(const void* x, int in_dtype, const float* gamma, const float* beta, void* out,
+                              int out_dtype, int B, int H, int W, int C, float eps, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(B > 0 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0 && C % 8 == 0,
                   "patch_merge_ln: need even H, W and C%%8==0 (H=%d W=%d C=%d)", H, W, C);
   PatchMergeRows map{x, out, H, W, C};
   return dispatch_ln(in_dtype, out_dtype, gamma, beta, (long)B * (H / 2) * (W / 2), 4 * C, eps, map, stream);
 }
 
-}  // namespace tfimm
+}  // extern "C"

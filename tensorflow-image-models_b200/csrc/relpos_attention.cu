@@ -400,9 +400,8 @@ int launch_relpos_bf16(const __nv_bfloat16* qkv, __nv_bfloat16* out, const __nv_
     return kUnsupported;
   }
   auto kernel = relpos_attention_bf16_kernel<DH>;
-  static unsigned long long attr_devs = 0;
-  if (first_use_on_device(attr_devs))
-    TFIMM_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 113 * 1024));
+  static std::atomic<unsigned long long> attr_devs{0};
+  TFIMM_CUDA_OK(set_max_dynamic_smem(kernel, 113 * 1024, attr_devs));
   dim3 grid((geo.N + kRpRows - 1) / kRpRows, H, B * geo.nseq);
   kernel<<<grid, kRpWarps * 32, smem, stream>>>(qkv, out, pad_bias, rel_h, rel_w, geo, H, scale * kLog2e, rs);
   TFIMM_LAUNCH_OK("relpos_attention_bf16_kernel");
@@ -411,8 +410,16 @@ int launch_relpos_bf16(const __nv_bfloat16* qkv, __nv_bfloat16* out, const __nv_
 
 }  // namespace
 
-int relpos_attention_bf16(const void* qkv, void* out, const void* pad_bias, const float* rel_h, const float* rel_w,
-                          int B, int gh, int gw, int H, int dh, int window, float scale, cudaStream_t stream) {
+}  // namespace tfimm
+
+using namespace tfimm;
+
+extern "C" {
+
+int tfimm_b200_relpos_attention_bf16(const void* qkv, void* out, const void* pad_bias, const float* rel_h,
+                                     const float* rel_w, int B, int gh, int gw, int H, int dh, int window, float scale,
+                                     void* s) {
+  const cudaStream_t stream = as_stream(s);
   RpGeom geo;
   if (int st = make_geom(geo, B, gh, gw, H, dh, window)) return st;
   TFIMM_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15u) == 0 && (reinterpret_cast<uintptr_t>(out) & 15u) == 0 &&
@@ -428,8 +435,10 @@ int relpos_attention_bf16(const void* qkv, void* out, const void* pad_bias, cons
   return kUnsupported;
 }
 
-int relpos_attention_f32(const float* qkv, float* out, const float* pad_bias, const float* rel_h, const float* rel_w,
-                         int B, int gh, int gw, int H, int dh, int window, float scale, cudaStream_t stream) {
+int tfimm_b200_relpos_attention_f32(const float* qkv, float* out, const float* pad_bias, const float* rel_h,
+                                    const float* rel_w, int B, int gh, int gw, int H, int dh, int window, float scale,
+                                    void* s) {
+  const cudaStream_t stream = as_stream(s);
   RpGeom geo;
   if (int st = make_geom(geo, B, gh, gw, H, dh, window)) return st;
   const int warps = 4;
@@ -438,10 +447,8 @@ int relpos_attention_f32(const float* qkv, float* out, const float* pad_bias, co
     set_last_error("relpos_attention_f32: sequence of %d tokens too long for the fp32 kernel", geo.N);
     return kUnsupported;
   }
-  static unsigned long long attr_devs = 0;
-  if (first_use_on_device(attr_devs))
-    TFIMM_CUDA_OK(cudaFuncSetAttribute(relpos_attention_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       227 * 1024));
+  static std::atomic<unsigned long long> attr_devs{0};
+  TFIMM_CUDA_OK(set_max_dynamic_smem(relpos_attention_f32_kernel, 227 * 1024, attr_devs));
   const long total = (long)B * geo.nseq * H * geo.N;
   const unsigned grid = (unsigned)((total + warps - 1) / warps);
   relpos_attention_f32_kernel<<<grid, warps * 32, smem, stream>>>(qkv, out, pad_bias, rel_h, rel_w, geo, H, dh, scale,
@@ -450,4 +457,4 @@ int relpos_attention_f32(const float* qkv, float* out, const float* pad_bias, co
   return kOk;
 }
 
-}  // namespace tfimm
+}  // extern "C"

@@ -196,8 +196,15 @@ __global__ void blur_pool_kernel(const T* __restrict__ x, T* __restrict__ out, l
 
 }  // namespace
 
-int grouped_conv(const void* x, int dtype, const float* wgt, const float* bias, void* out, int B, int H, int W,
-                 int C, int cg, int ks, int stride, int pad, int Ho, int Wo, int act, cudaStream_t stream) {
+}  // namespace tfimm
+
+using namespace tfimm;
+
+extern "C" {
+
+int tfimm_b200_grouped_conv(const void* x, int dtype, const float* wgt, const float* bias, void* out, int B, int H,
+                            int W, int C, int cg, int ks, int stride, int pad, int Ho, int Wo, int act, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(B > 0 && C > 0 && cg > 0 && C % cg == 0, "grouped_conv: bad channel grouping (C=%d cg=%d)", C, cg);
   TFIMM_CHECK_ARG(dtype == kBF16 || dtype == kF32, "grouped_conv: dtype must be bf16 or f32");
   const long total = (long)B * Ho * Wo * (C / cg);
@@ -225,15 +232,17 @@ int grouped_conv(const void* x, int dtype, const float* wgt, const float* bias, 
   return kOk;
 }
 
-int eca_gate(const float* mean, const float* w, float* gate, int B, int C, int ks, cudaStream_t stream) {
+int tfimm_b200_eca_gate(const float* mean, const float* w, float* gate, int B, int C, int ks, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(B > 0 && C > 0 && ks > 0 && (ks & 1), "eca_gate: need an odd kernel size");
   eca_gate_kernel<<<rgrid((long)B * C, 256), 256, 0, stream>>>(mean, w, gate, B, C, ks);
   TFIMM_LAUNCH_OK("eca_gate_kernel");
   return kOk;
 }
 
-int scale_add_act(void* x, int dtype, const float* gate, const void* shortcut, int B, int HW, int C, int act,
-                  cudaStream_t stream) {
+int tfimm_b200_scale_add_act(void* x, int dtype, const float* gate, const void* shortcut, int B, int HW, int C, int act,
+                             void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(B > 0 && HW > 0 && C % 8 == 0, "scale_add_act: need C%%8==0 (C=%d)", C);
   const long total = (long)B * HW * (C / 8);
   if (dtype == kBF16)
@@ -250,8 +259,9 @@ int scale_add_act(void* x, int dtype, const float* gate, const void* shortcut, i
   return kOk;
 }
 
-int group_norm(const void* x, int dtype, const float* gamma, const float* beta, const void* residual, void* out,
-               float* stats, int B, int HW, int C, int groups, float eps, int act, cudaStream_t stream) {
+int tfimm_b200_group_norm(const void* x, int dtype, const float* gamma, const float* beta, const void* residual,
+                          void* out, float* stats, int B, int HW, int C, int groups, float eps, int act, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(B > 0 && HW > 0 && groups > 0 && C % groups == 0 && C % 8 == 0,
                   "group_norm: need C%%groups==0 and C%%8==0 (C=%d groups=%d)", C, groups);
   const long total = (long)B * HW * (C / 8);
@@ -271,8 +281,9 @@ int group_norm(const void* x, int dtype, const float* gamma, const float* beta, 
   return kOk;
 }
 
-int blur_pool(const void* x, int dtype, void* out, int B, int H, int W, int C, int stride, int Ho, int Wo,
-              cudaStream_t stream) {
+int tfimm_b200_blur_pool(const void* x, int dtype, void* out, int B, int H, int W, int C, int stride, int Ho, int Wo,
+                         void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(B > 0 && H > 1 && W > 1 && C % 8 == 0 && stride > 0, "blur_pool: need H,W>1 and C%%8==0 (C=%d)", C);
   const long total = (long)B * Ho * Wo * (C / 8);
   if (dtype == kBF16)
@@ -289,4 +300,4 @@ int blur_pool(const void* x, int dtype, void* out, int B, int H, int W, int C, i
   return kOk;
 }
 
-}  // namespace tfimm
+}  // extern "C"

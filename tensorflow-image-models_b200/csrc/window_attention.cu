@@ -191,9 +191,8 @@ int launch_window_attention(const void* qkv, void* out, const float* bias, const
   const unsigned grid = (unsigned)((pairs + kWWarps - 1) / kWWarps);
   constexpr int smem = kWWarps * 3 * ROWS * kWDH * 2;   // 48 KB / 108 KB (two CTAs per SM)
   auto kernel = window_attention_bf16_kernel<ROWS, kPadded>;
-  static unsigned long long attr_devs = 0;
-  if (first_use_on_device(attr_devs))
-    TFIMM_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  static std::atomic<unsigned long long> attr_devs{0};
+  TFIMM_CUDA_OK(set_max_dynamic_smem(kernel, smem, attr_devs));
   kernel<<<grid, kWWarps * 32, smem, stream>>>(reinterpret_cast<const __nv_bfloat16*>(qkv),
                                                reinterpret_cast<__nv_bfloat16*>(out), bias, row_map, labels, maskbits,
                                                pairs, nw_img, N, H, scale);
@@ -203,9 +202,15 @@ int launch_window_attention(const void* qkv, void* out, const float* bias, const
 
 }  // namespace
 
-int window_attention_bf16(const void* qkv, void* out, const float* bias, const int* row_map,
-                          const int* labels, int B, int nw_img, int N, int H, int dh, float scale,
-                          cudaStream_t stream) {
+}  // namespace tfimm
+
+using namespace tfimm;
+
+extern "C" {
+
+int tfimm_b200_window_attention_bf16(const void* qkv, void* out, const float* bias, const int* row_map,
+                                     const int* labels, int B, int nw_img, int N, int H, int dh, float scale, void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(B > 0 && nw_img > 0 && N > 0 && H > 0, "window_attention: bad shape");
   TFIMM_CHECK_ARG(bias != nullptr && row_map != nullptr, "window_attention: bias and row_map are required");
   if (dh != kWDH || N > 144) {
@@ -219,9 +224,10 @@ int window_attention_bf16(const void* qkv, void* out, const float* bias, const i
 
 // bias_pad: [H][64][64] fp32 (rows / columns beyond N are ignored); maskbits: [nw_img][64] uint64, bit j of entry
 // (wi, i) set when tokens i and j of window wi lie in different shift regions (null for unshifted blocks).
-int window_attention_tc_bf16(const void* qkv, void* out, const float* bias_pad, const int* row_map,
-                             const unsigned long long* maskbits, int B, int nw_img, int N, int H, int dh, float scale,
-                             cudaStream_t stream) {
+int tfimm_b200_window_attention_tc_bf16(const void* qkv, void* out, const float* bias_pad, const int* row_map,
+                                        const void* maskbits, int B, int nw_img, int N, int H, int dh, float scale,
+                                        void* s) {
+  const cudaStream_t stream = as_stream(s);
   TFIMM_CHECK_ARG(B > 0 && nw_img > 0 && N > 0 && H > 0, "window_attention: bad shape");
   TFIMM_CHECK_ARG(bias_pad != nullptr && row_map != nullptr, "window_attention: bias and row_map are required");
   if (dh != kWDH || N > 52) {
@@ -232,8 +238,9 @@ int window_attention_tc_bf16(const void* qkv, void* out, const float* bias_pad, 
   TFIMM_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15u) == 0 && (reinterpret_cast<uintptr_t>(out) & 15u) == 0 &&
                       (reinterpret_cast<uintptr_t>(bias_pad) & 15u) == 0,
                   "window_attention: qkv / out / bias must be 16-byte aligned");
-  return launch_window_attention<64, true>(qkv, out, bias_pad, row_map, nullptr, maskbits, B, nw_img, N, H, scale,
+  return launch_window_attention<64, true>(qkv, out, bias_pad, row_map, nullptr,
+                                           static_cast<const unsigned long long*>(maskbits), B, nw_img, N, H, scale,
                                            stream);
 }
 
-}  // namespace tfimm
+}  // extern "C"

@@ -44,7 +44,7 @@ def token_gemm(wt, x, bias=None, act=None, gamma=None, residual=None, mul=None, 
     Epilogue: + bias[m] -> act (glu: rows in ``glu_interleave`` order, value * act(gate)) -> * gamma[c] -> * mul[b, row,
     c] -> + residual[b, row, c] (may be ``out``).  Rows >= m_out are not stored.  out / residual / mul: (B, m_out, C)
     with unit channel stride.  bf16 x: wgmma (out bf16 or fp32); fp32 x: CUDA cores."""
-    _ops._cuda(wt, x, bias, gamma, residual, mul, out)
+    dev = _ops._cuda(wt, x, bias, gamma, residual, mul, out)
     B, K, C = x.shape
     M = wt.shape[0]
     ldw = wt.stride(0)
@@ -69,17 +69,14 @@ def token_gemm(wt, x, bias=None, act=None, gamma=None, residual=None, mul=None, 
     (ldr, img_r), (ldu, img_u), (ldc, img_c) = st(residual), st(mul), st(out)
     flops = 2.0 * B * M * K * C
     nbytes = _ops._nbytes(wt, x, out, residual, mul)
+    args = (wt.data_ptr(), ldw, x.data_ptr(), x.stride(1), x.stride(0), _ops._ptr(bias), _ops._ptr(gamma),
+            _ops._ptr(residual), ldr, img_r, _ops._ptr(mul), ldu, img_u, out.data_ptr(), ldc, img_c, B, M, C, K, m_out,
+            _ops.act_code(act), int(glu))
     if x.dtype == torch.bfloat16:
-        _ops._call("tfimm_b200_token_gemm_bf16", wt.data_ptr(), ldw, x.data_ptr(), x.stride(1), x.stride(0),
-                   _ops._ptr(bias), _ops._ptr(gamma), _ops._ptr(residual), ldr, img_r, _ops._ptr(mul), ldu, img_u,
-                   out.data_ptr(), ldc, img_c, B, M, C, K, m_out, _ops.act_code(act), int(glu), _ops._code(out),
-                   block_n, _ops._stream(), flops=flops, nbytes=nbytes)
+        _ops._call("tfimm_b200_token_gemm_bf16", dev, *args, _ops._code(out), block_n, flops=flops, nbytes=nbytes)
     elif x.dtype == torch.float32:
         assert out.dtype == torch.float32
-        _ops._call("tfimm_b200_token_gemm_f32", wt.data_ptr(), ldw, x.data_ptr(), x.stride(1), x.stride(0),
-                   _ops._ptr(bias), _ops._ptr(gamma), _ops._ptr(residual), ldr, img_r, _ops._ptr(mul), ldu, img_u,
-                   out.data_ptr(), ldc, img_c, B, M, C, K, m_out, _ops.act_code(act), int(glu), _ops._stream(),
-                   flops=flops, nbytes=nbytes)
+        _ops._call("tfimm_b200_token_gemm_f32", dev, *args, flops=flops, nbytes=nbytes)
     else:
         raise _lib.KernelLibraryError(f"token_gemm: unsupported dtype {x.dtype}")
     return out
@@ -88,7 +85,7 @@ def token_gemm(wt, x, bias=None, act=None, gamma=None, residual=None, mul=None, 
 def gemm_glu(a, w, bias, n_out, act, block_n=0):
     """Channel GLU: (a @ w_value.T + b) * act(a @ w_gate.T + b) -> (M, n_out), with w / bias in ``glu_interleave`` order
     (bf16: axis_rows=False, fp32: axis_rows=True).  The full-width hidden tensor is never written."""
-    _ops._cuda(a, w, bias)
+    dev = _ops._cuda(a, w, bias)
     M, K = a.shape
     N = w.shape[0]
     assert w.shape[1] == K and a.stride(1) == 1 and w.stride(1) == 1 and a.dtype == w.dtype
@@ -96,16 +93,13 @@ def gemm_glu(a, w, bias, n_out, act, block_n=0):
     ldc = _ceil(n_out, 8)
     buf = torch.empty((M, ldc), device=a.device, dtype=a.dtype)
     out = buf[:, :n_out] if ldc != n_out else buf
-    flops = 2.0 * M * N * K
+    flops, nbytes = 2.0 * M * N * K, _ops._nbytes(a, w, out)
+    args = (a.data_ptr(), a.stride(0), w.data_ptr(), w.stride(0), bias.data_ptr(), out.data_ptr(), ldc, M, N)
     if a.dtype == torch.bfloat16:
         assert N == 2 * n_out
-        _ops._call("tfimm_b200_gemm_glu_bf16", a.data_ptr(), a.stride(0), w.data_ptr(), w.stride(0), bias.data_ptr(),
-                   out.data_ptr(), ldc, M, N, K, _ops.act_code(act), block_n, _ops._stream(), flops=flops,
-                   nbytes=_ops._nbytes(a, w, out))
+        _ops._call("tfimm_b200_gemm_glu_bf16", dev, *args, K, _ops.act_code(act), block_n, flops=flops, nbytes=nbytes)
     elif a.dtype == torch.float32:
-        _ops._call("tfimm_b200_gemm_glu_f32", a.data_ptr(), a.stride(0), w.data_ptr(), w.stride(0), bias.data_ptr(),
-                   out.data_ptr(), ldc, M, N, n_out, K, _ops.act_code(act), _ops._stream(), flops=flops,
-                   nbytes=_ops._nbytes(a, w, out))
+        _ops._call("tfimm_b200_gemm_glu_f32", dev, *args, n_out, K, _ops.act_code(act), flops=flops, nbytes=nbytes)
     else:
         raise _lib.KernelLibraryError(f"gemm_glu: unsupported dtype {a.dtype}")
     return out
@@ -113,11 +107,11 @@ def gemm_glu(a, w, bias, n_out, act, block_n=0):
 
 def affine(x, alpha, beta, out_dtype):
     """ResMLP's Affine norm alpha[c] x + beta[c] of a 2-D fp32 x (unit column stride) -> (rows, C) in out_dtype."""
-    _ops._cuda(x, alpha, beta)
+    dev = _ops._cuda(x, alpha, beta)
     rows, C = x.shape
     assert x.dtype == torch.float32 and x.stride(1) == 1
     assert alpha.shape == beta.shape == (C,) and alpha.dtype == beta.dtype == torch.float32
     out = torch.empty((rows, C), device=x.device, dtype=out_dtype)
-    _ops._call("tfimm_b200_affine", x.data_ptr(), x.stride(0), alpha.data_ptr(), beta.data_ptr(), out.data_ptr(),
-               _ops._code(out), out.stride(0), rows, C, _ops._stream(), nbytes=_ops._nbytes(x, out))
+    _ops._call("tfimm_b200_affine", dev, x.data_ptr(), x.stride(0), alpha.data_ptr(), beta.data_ptr(), out.data_ptr(),
+               _ops._code(out), out.stride(0), rows, C, nbytes=_ops._nbytes(x, out))
     return out

@@ -26,7 +26,7 @@ def relpos_attention(qkv, B, gh, gw, H, dh, scale, rel_h, rel_w, window=0, pad_b
     of the window, whose padding positions are keys with k / v from ``pad_bias`` (the qkv bias, (3*H*dh,), same dtype
     as qkv; None: zero keys).  rel_h / rel_w: fp32 (2*S - 1, dh) tables of the sequence extent S (window, or gh / gw).
     bf16 qkv: tensor-core kernel (head_dim 64 / 80); fp32 qkv: SIMT kernel."""
-    _ops._cuda(qkv, rel_h, rel_w, pad_bias)
+    dev = _ops._cuda(qkv, rel_h, rel_w, pad_bias)
     N = gh * gw
     sh, sw = (window, window) if window else (gh, gw)
     assert qkv.shape == (B * N, 3 * H * dh) and qkv.is_contiguous(), (qkv.shape, B, N, H, dh)
@@ -38,11 +38,11 @@ def relpos_attention(qkv, B, gh, gw, H, dh, scale, rel_h, rel_w, window=0, pad_b
     nseq = (-(-gh // sh)) * (-(-gw // sw))
     flops = 4.0 * B * nseq * H * (sh * sw) ** 2 * dh
     args = (qkv.data_ptr(), out.data_ptr(), _ops._ptr(pad_bias), rel_h.data_ptr(), rel_w.data_ptr(), B, gh, gw, H, dh,
-            int(window), float(scale), _ops._stream())
+            int(window), float(scale))
     if qkv.dtype == torch.bfloat16:
-        _ops._call("tfimm_b200_relpos_attention_bf16", *args, flops=flops, nbytes=_ops._nbytes(qkv, out))
+        _ops._call("tfimm_b200_relpos_attention_bf16", dev, *args, flops=flops, nbytes=_ops._nbytes(qkv, out))
     elif qkv.dtype == torch.float32:
-        _ops._call("tfimm_b200_relpos_attention_f32", *args, flops=flops, nbytes=_ops._nbytes(qkv, out))
+        _ops._call("tfimm_b200_relpos_attention_f32", dev, *args, flops=flops, nbytes=_ops._nbytes(qkv, out))
     else:
         raise _lib.KernelLibraryError(f"relpos_attention: unsupported dtype {qkv.dtype}")
     return out
