@@ -413,6 +413,23 @@ int pick_block_n(int M, int N) {
   return best;
 }
 
+// Tile width of the plain bf16 GEMM (tfimm_b200_gemm_bf16), from its wave count and a per-wave time fitted to
+// measurements of that kernel (profiles/gemm_h100.md).  The other instances keep pick_block_n: their kernels (A-transform
+// warps, TF32 k-blocks, token mixing) were not measured against this model.
+//   BLOCK_N = 128, one CTA per SM: the epilogue runs after the mainloop with the tensor cores idle, so a wave costs
+//     ~ 128 * (K + kEpilogueK).
+//   BLOCK_N = 64, two CTAs per SM: one CTA's epilogue runs under the other's mainloop, so a wave of two tiles per SM
+//     costs ~ kPairWidth * K.
+// BLOCK_N = 256 is not chosen: it was the slowest width at every measured shape (force_block_n still selects it).
+int pick_block_n_bf16(int M, int N, int K) {
+  constexpr double kEpilogueK = 926.0, kPairWidth = 184.0;
+  const int sms = sm_count() > 0 ? sm_count() : 132;  // no device (host-side shape queries): H100 SXM
+  const long mt = (M + kBlockM - 1) / kBlockM;
+  const long waves128 = (mt * ((N + 127) / 128) + sms - 1) / sms;
+  const long waves64 = (mt * ((N + 63) / 64) + 2 * sms - 1) / (2 * sms);
+  return (double)waves64 * kPairWidth * K < (double)waves128 * 128.0 * (K + kEpilogueK) ? 64 : 128;
+}
+
 }  // namespace
 
 int gemm_bf16_skinny(const void* A, int lda, const void* W, int ldw, const float* bias, const void* residual, int ldr,
@@ -470,7 +487,7 @@ int tfimm_b200_gemm_bf16(const void* A, int lda, const void* W, int ldw, const f
   p.M = M; p.N = N; p.K = K;
   p.bias = bias; p.gamma = gamma; p.act = act; p.has_res = residual != nullptr ? 1 : 0; p.act_post = act_post;
   // force_block_n: 0 = choose; 64/128/256 = that tile width; 2 = the widest tile (256)
-  const int bn = force_block_n == 2 ? 256 : (force_block_n > 0 ? force_block_n : pick_block_n(M, N));
+  const int bn = force_block_n == 2 ? 256 : (force_block_n > 0 ? force_block_n : pick_block_n_bf16(M, N, K));
   return with_block_n<256>(bn, "gemm: unsupported block_n %d", [&](auto n) {
     constexpr int BN = decltype(n)::value;
     return out_dtype == kBF16 ? launch_gemm<BN, __nv_bfloat16>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream)
