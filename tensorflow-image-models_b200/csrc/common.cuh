@@ -413,6 +413,13 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
+// Named barrier kId (1..15; 0 is __syncthreads) over `threads` threads, a multiple of 32.  The id is an immediate so
+// that ptxas reserves only the barriers a kernel names.
+template <int kId>
+__device__ __forceinline__ void named_bar_sync(int threads) {
+  asm volatile("bar.sync %0, %1;" ::"n"(kId), "r"(threads) : "memory");
+}
+
 __device__ __forceinline__ void prefetch_tmap(const void* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmap)) : "memory");
 }

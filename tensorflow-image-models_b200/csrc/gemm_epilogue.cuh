@@ -1,6 +1,7 @@
 // Epilogue shared by the wgmma GEMM kernels (gemm_sm90.cu, the fc2 half of mlp_sm90.cu):
 //     C = residual + gamma * act(acc + bias)            (or act(residual + ...) with act_post)
-// applied straight to a warpgroup's accumulator fragments (wgmma.cuh): each thread owns two rows (r, r + 8) and, per
+// epilogue_staged (plain GEMM) goes through a shared-memory tile with TMA in and out; epilogue_frag works on global
+// memory straight from a warpgroup's accumulator fragments (wgmma.cuh).  In both, each thread owns two rows (r, r + 8) and, per
 // 8-column group, two adjacent columns of each, so bias / gamma / activation run on packed fp32 pairs and the residual
 // load and output store are one 4- or 8-byte access per row and group.  The residual may alias the output (in-place
 // fp32 residual stream): every element is read and written by the same thread.
@@ -130,9 +131,14 @@ __device__ __forceinline__ void st_out_pair(__nv_bfloat16* p, uint64_t v, bool t
 // Epilogue of one warpgroup's 64 x BN accumulator (BN / 2 fp32 per thread, wgmma.cuh layout) of tile (m_blk, n_blk);
 // the warpgroup's rows start at tile row `wg_row0`.  Columns are handled 8 at a time (four values per thread: rows r and
 // r + 8, columns c and c + 1), which is the granularity of the four-element activations.
+// The groups go in runs of kRun: the bias, gamma and residual loads of a whole run are issued before its first store, so
+// they overlap instead of each waiting behind the previous group's store (the residual may alias C, so the compiler
+// cannot move a load above a store; loading ahead is legal because every element is read and written by the same
+// thread).  kRun bounds the registers the loads hold: the 256-wide instances have the fewest to spare.
 template <typename OutT, int BN>
 __device__ __forceinline__ void epilogue_frag(const GemmParams& p, float (&acc)[BN / 2], int m_blk, int n_blk,
                                               int wg_row0) {
+  constexpr int kRun = BN >= 256 ? 2 : 4;
   const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
   const int r = wg_row0 + wq * 16 + (lane >> 2);
   const long off_c[2] = {epilogue_row_offset(p, m_blk, r, p.ldc), epilogue_row_offset(p, m_blk, r + 8, p.ldc)};
@@ -141,31 +147,142 @@ __device__ __forceinline__ void epilogue_frag(const GemmParams& p, float (&acc)[
   OutT* __restrict__ C = reinterpret_cast<OutT*>(p.c);
   const OutT* R = reinterpret_cast<const OutT*>(p.res);
 #pragma unroll
+  for (int g0 = 0; g0 < BN / 8; g0 += kRun) {
+    if (n_blk * BN + g0 * 8 >= p.N) break;
+    uint64_t b[kRun], s[kRun], res[kRun][2];
+#pragma unroll
+    for (int j = 0; j < kRun; ++j) {
+      const int n = n_blk * BN + (g0 + j) * 8 + 2 * (lane & 3);
+      const bool in = n < p.N, two = n + 1 < p.N;
+      b[j] = p.bias != nullptr ? ld_pair_or(p.bias, n, p.N, 0.f) : 0;
+      s[j] = p.gamma != nullptr ? ld_pair_or(p.gamma, n, p.N, 1.f) : 0;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        res[j][h] = p.has_res && in && off_r[h] >= 0 ? ld_out_pair(R + off_r[h] + n, two) : 0;
+    }
+#pragma unroll
+    for (int j = 0; j < kRun; ++j) {
+      const int g = g0 + j;
+      const int n = n_blk * BN + g * 8 + 2 * (lane & 3);
+      if (n_blk * BN + g * 8 >= p.N) break;
+      const bool in = n < p.N, two = n + 1 < p.N;
+      uint64_t v[2] = {pack2(acc[4 * g + 0], acc[4 * g + 1]), pack2(acc[4 * g + 2], acc[4 * g + 3])};
+      if (p.bias != nullptr) {
+        v[0] = add2(v[0], b[j]);
+        v[1] = add2(v[1], b[j]);
+      }
+      if (!p.act_post) apply_act_pairs(v, p.act);
+      if (p.gamma != nullptr) {
+        v[0] = mul2(v[0], s[j]);
+        v[1] = mul2(v[1], s[j]);
+      }
+      if (p.has_res) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          if (in && off_r[h] >= 0) v[h] = add2(v[h], res[j][h]);
+      }
+      if (p.act_post) apply_act_pairs(v, p.act);
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        if (in && off_c[h] >= 0) st_out_pair(C + off_c[h] + n, v[h], two);
+    }
+  }
+}
+
+// ---- staged epilogue (plain GEMM, gemm_sm90.cu) ----
+// The 128 x BN output tile lives in shared memory as column chunks of one 128-byte swizzle span (64 bf16 or 32 fp32
+// columns); each warpgroup's 64 rows of a chunk are one 8 KB SWIZZLE_128B box, the layout TMA loads the residual into
+// and stores the result from.  Box (wg, chunk) is at chunk_base + (wg * kChunks + chunk) * 8192.
+template <typename OutT>
+constexpr int staged_chunk_cols() { return 128 / (int)sizeof(OutT); }
+constexpr int kStagedBoxBytes = 64 * 128;
+
+// Shared-memory address of the pair (row, col), (row, col + 1) of a warpgroup's staged rows.  16-byte unit u of row r
+// sits at unit u ^ (r & 7), so a warp's access for one column group (8 rows x 4 pairs) takes the fewest wavefronts
+// its size allows: one for bf16 pairs (128 bytes), two for fp32 pairs (256 bytes).
+template <typename OutT>
+__device__ __forceinline__ uint32_t staged_addr(uint32_t s_wg, int row, int col) {
+  constexpr int kCols = staged_chunk_cols<OutT>();
+  const uint32_t byte = (uint32_t)(col % kCols) * (uint32_t)sizeof(OutT);
+  return s_wg + (uint32_t)(col / kCols) * kStagedBoxBytes + (uint32_t)row * 128u +
+         ((((byte >> 4) ^ (uint32_t)(row & 7)) << 4) | (byte & 15u));
+}
+__device__ __forceinline__ uint64_t ld_staged_pair(const float*, uint32_t a) {
+  float x, y;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(x), "=f"(y) : "r"(a) : "memory");
+  return pack2(x, y);
+}
+__device__ __forceinline__ uint64_t ld_staged_pair(const __nv_bfloat16*, uint32_t a) {
+  uint32_t u;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(u) : "r"(a) : "memory");
+  const float2 f = unpack_bf16x2(u);
+  return pack2(f.x, f.y);
+}
+__device__ __forceinline__ void st_staged_pair(float*, uint32_t a, uint64_t v) {
+  float x, y;
+  unpack2(v, x, y);
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(x), "f"(y) : "memory");
+}
+__device__ __forceinline__ void st_staged_pair(__nv_bfloat16*, uint32_t a, uint64_t v) {
+  float x, y;
+  unpack2(v, x, y);
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(pack_bf16x2(x, y)) : "memory");
+}
+
+// Epilogue of one warpgroup (rows 64 wg .. 64 wg + 63 of tile (m_blk, n_blk)) through the staged tile s_out.  The
+// per-element fp32 operations are those of epilogue_frag, in the same order.  s_bias / s_gamma hold the tile's BN
+// bias and gamma values, written by the consumer threads before their mainloop; res_bar completes when the residual
+// tile has landed in s_out (p.has_res).  Each element is read from and written back to s_out by the same thread, so
+// the residual may alias C: the TMA store of the tile is issued only after its residual load has completed.  The
+// output tensor map has the real extents (N, M), so the store clips the M and N tails.
+template <typename OutT, int BN>
+__device__ __forceinline__ void epilogue_staged(const GemmParams& p, float (&acc)[BN / 2], int m_blk, int n_blk, int wg,
+                                                uint32_t s_out, const float* s_bias, const float* s_gamma,
+                                                uint32_t res_bar, const CUtensorMap* tmap_c) {
+  constexpr int kCols = staged_chunk_cols<OutT>(), kChunks = BN / kCols;
+  const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
+  const int r = wq * 16 + (lane >> 2);   // warpgroup row; r + 8 has the same swizzle phase
+  const uint32_t s_wg = s_out + (uint32_t)(wg * kChunks * kStagedBoxBytes);
+  OutT* const tag = nullptr;
+  named_bar_sync<1>(256);   // s_bias / s_gamma were written by both consumer warpgroups
+  if (p.has_res) mbar_wait(res_bar, 0);
+#pragma unroll
   for (int g = 0; g < BN / 8; ++g) {
-    const int n = n_blk * BN + g * 8 + 2 * (lane & 3);
-    if (n_blk * BN + g * 8 >= p.N) break;
-    const bool in = n < p.N, two = n + 1 < p.N;
+    const int c = g * 8 + 2 * (lane & 3);
+    const uint32_t a0 = staged_addr<OutT>(s_wg, r, c), a1 = a0 + 8 * 128;
     uint64_t v[2] = {pack2(acc[4 * g + 0], acc[4 * g + 1]), pack2(acc[4 * g + 2], acc[4 * g + 3])};
     if (p.bias != nullptr) {
-      const uint64_t b = ld_pair_or(p.bias, n, p.N, 0.f);
-      v[0] = add2(v[0], b);
-      v[1] = add2(v[1], b);
+      const float2 b = *reinterpret_cast<const float2*>(s_bias + c);
+      v[0] = add2(v[0], pack2(b.x, b.y));
+      v[1] = add2(v[1], pack2(b.x, b.y));
     }
     if (!p.act_post) apply_act_pairs(v, p.act);
     if (p.gamma != nullptr) {
-      const uint64_t s = ld_pair_or(p.gamma, n, p.N, 1.f);
-      v[0] = mul2(v[0], s);
-      v[1] = mul2(v[1], s);
+      const float2 s = *reinterpret_cast<const float2*>(s_gamma + c);
+      v[0] = mul2(v[0], pack2(s.x, s.y));
+      v[1] = mul2(v[1], pack2(s.x, s.y));
     }
     if (p.has_res) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-        if (in && off_r[h] >= 0) v[h] = add2(v[h], ld_out_pair(R + off_r[h] + n, two));
+      v[0] = add2(v[0], ld_staged_pair(tag, a0));
+      v[1] = add2(v[1], ld_staged_pair(tag, a1));
     }
     if (p.act_post) apply_act_pairs(v, p.act);
+    st_staged_pair(tag, a0, v[0]);
+    st_staged_pair(tag, a1, v[1]);
+  }
+  // generic-proxy writes -> visible to the TMA engine, then one thread stores the warpgroup's rows
+  fence_proxy_async_smem();
+  if (wg == 0) named_bar_sync<2>(128);
+  else named_bar_sync<3>(128);
+  const int row0 = m_blk * 128 + wg * 64;
+  if ((threadIdx.x & 127) == 0 && row0 < p.M) {
 #pragma unroll
-    for (int h = 0; h < 2; ++h)
-      if (in && off_c[h] >= 0) st_out_pair(C + off_c[h] + n, v[h], two);
+    for (int ch = 0; ch < kChunks; ++ch) {
+      const int col0 = n_blk * BN + ch * kCols;
+      if (col0 < p.N) tma_store_2d(tmap_c, s_wg + (uint32_t)(ch * kStagedBoxBytes), col0, row0);
+    }
+    tma_store_commit();
+    tma_store_wait_read<0>();   // the tile must not be released before the TMA engine has read it
   }
 }
 

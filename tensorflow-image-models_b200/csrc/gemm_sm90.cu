@@ -12,8 +12,10 @@
 // Design (one 128 x BLOCK_N output tile per CTA, warp-specialised):
 //   warps 0..7  two consumer warpgroups, 64 tile rows each: wgmma m64 x BLOCK_N x k16 from the swizzled smem ring,
 //               fp32 accumulators in registers, one wgmma group kept in flight (the stage of the group before it is
-//               released as soon as it retires); then the epilogue straight from the fragments (gemm_epilogue.cuh)
-//   warp 8      TMA producer: A/W tiles -> 128B-swizzled smem ring (mbarrier full/empty)
+//               released as soon as it retires); then the epilogue (gemm_epilogue.cuh): staged through shared memory
+//               with TMA residual load and output store (plain bf16 GEMM, BLOCK_N <= 128), or from the fragments
+//   warp 8      TMA producer: A/W tiles -> 128B-swizzled smem ring (mbarrier full/empty); the residual tile of the
+//               staged epilogue
 //   warps 9..12 (A-transform instances only) rewrite the A tile in smem before the MMA reads it: the squeeze-excite
 //               gate (bf16), or the TF32 rounding of fp32 activations (precision="tf32")
 //
@@ -58,14 +60,26 @@ constexpr int block_k() { return kRowBytes / (int)sizeof(OperandT<AX>); }   // 6
 template <int AX>
 constexpr int dtype_code() { return AX == kATf32 ? kF32 : kBF16; }
 
-template <int BLOCK_N>
+// STAGED (plain bf16 GEMM at BLOCK_N 64 / 128, epilogue_staged): after the ring, a 128 x BLOCK_N OutT tile that takes
+// the residual by TMA during the mainloop and holds the result for the TMA store, then the tile's bias and gamma.
+// Shared memory per CTA (ring + tile + bias / gamma + barriers + alignment slack; the SM reserves 1 KB more per CTA,
+// and has 228 KB in all):
+//   BLOCK_N = 64:  4 stages = 96 KB, or 3 stages = 72 KB + 16 / 32 KB (bf16 / fp32 tile) when STAGED: two CTAs per SM
+//                  either way (4 stages + a 16 KB tile would need 2 x 114.6 KB with the reserved 1 KB)
+//   BLOCK_N = 128: 4 stages = 128 KB, + 32 / 64 KB when STAGED: one CTA per SM
+//   BLOCK_N = 256: 4 stages = 192 KB, no room for a tile: fragment epilogue only
+template <int BLOCK_N, typename OutT = float, bool STAGED = false>
 struct GemmCfg {
   static constexpr int kABytes = kBlockM * kRowBytes;
   static constexpr int kBBytes = BLOCK_N * kRowBytes;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStages = 4;   // 192 / 128 / 96 KB: BLOCK_N = 64 leaves room for two CTAs per SM
-  static constexpr int kNumBarriers = 3 * kStages;   // full, empty, ready (A-transform instances)
-  static constexpr int kSmemBytes = kStages * kStageBytes + kNumBarriers * 8 + 1024 /*alignment slack*/;
+  static constexpr int kStages = STAGED && BLOCK_N == 64 ? 3 : 4;
+  static constexpr int kOutBytes = STAGED ? kBlockM * BLOCK_N * (int)sizeof(OutT) : 0;
+  static constexpr int kVecBytes = STAGED ? 2 * BLOCK_N * 4 : 0;   // bias, gamma
+  static constexpr int kNumBarriers = 3 * kStages + 1;   // full, empty, ready (A-transform instances), residual
+  static constexpr int kSmemBytes =
+      kStages * kStageBytes + kOutBytes + kVecBytes + kNumBarriers * 8 + 1024 /*alignment slack*/;
+  static_assert(!STAGED || BLOCK_N <= 128, "the staged epilogue's tile does not fit next to a 256-wide ring");
 };
 
 // B operand descriptor: K-major, or MN-major for token mixing; one k16 step is 32 bytes (+2) or 16 MN-major rows (+128).
@@ -80,11 +94,15 @@ constexpr int kDescStepB = kMN ? 128 : 2;
 template <int BLOCK_N, int AX>
 constexpr int gemm_threads() { return kConsumerThreads + 32 + (AX != kANone ? 32 * kNumGateWarps : 0); }
 
-template <int BLOCK_N, typename OutT, int AX = kANone, int MODE = kModeGemm>
+// STAGED: epilogue_staged, with the output (tmap_c) and residual (tmap_r) tensor maps; otherwise they are unused and
+// the epilogue works from the fragments.
+template <int BLOCK_N, typename OutT, int AX = kANone, int MODE = kModeGemm, bool STAGED = false>
 __global__ void __launch_bounds__(gemm_threads<BLOCK_N, AX>(), (BLOCK_N == 64 && AX == kANone) ? 2 : 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                       const GemmParams p) {
-  using Cfg = GemmCfg<BLOCK_N>;
+                  const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ CUtensorMap tmap_r,
+                  const GemmParams p) {
+  static_assert(!STAGED || (AX == kANone && MODE == kModeGemm), "staged epilogue: plain bf16 GEMM only");
+  using Cfg = GemmCfg<BLOCK_N, OutT, STAGED>;
   constexpr int kStages = Cfg::kStages;
   constexpr int kBlockK = block_k<AX>();
 
@@ -92,10 +110,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   // SWIZZLE_128B tiles need 1024-byte alignment.
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t smem_tiles = smem_base;
-  const uint32_t smem_bars = smem_base + kStages * Cfg::kStageBytes;
+  const uint32_t smem_out = smem_base + kStages * Cfg::kStageBytes;
+  const uint32_t smem_vec = smem_out + Cfg::kOutBytes;
+  const uint32_t smem_bars = smem_vec + Cfg::kVecBytes;
   auto full_bar = [&](int s) { return smem_bars + 8u * s; };
   auto empty_bar = [&](int s) { return smem_bars + 8u * (kStages + s); };
   auto ready_bar = [&](int s) { return smem_bars + 8u * (2 * kStages + s); };
+  const uint32_t res_bar = smem_bars + 8u * (3 * kStages);
+  float* const s_bias = reinterpret_cast<float*>(smem_raw + (smem_vec - smem_u32(smem_raw)));
+  float* const s_gamma = s_bias + BLOCK_N;
 
   const int warp_idx = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -103,6 +126,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   if (warp_idx == kProducerWarp && lane == 0) {
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_b);
+    if constexpr (STAGED) {
+      prefetch_tmap(&tmap_c);
+      if (p.has_res) prefetch_tmap(&tmap_r);
+      mbar_init(res_bar, 1);
+    }
     for (int s = 0; s < kStages; ++s) {
       mbar_init(full_bar(s), 1);
       mbar_init(empty_bar(s), 2);   // one arrival per consumer warpgroup
@@ -135,7 +163,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         const uint32_t sa = smem_tiles + stage * Cfg::kStageBytes;
         const uint32_t sb = sa + Cfg::kABytes;
         mbar_expect_tx(full_bar(stage), Cfg::kStageBytes);
-        if (p.conv == 0) {
+        if (STAGED || p.conv == 0) {
           tma_load_2d(sa, &tmap_a, full_bar(stage), kb * kBlockK, m_blk * kBlockM);
         } else {
           // implicit convolution: tap (ky, kx) and a kBlockK-channel slice of the input patch; padding = OOB zero fill
@@ -152,6 +180,20 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             tma_load_3d(sb + i * 8192, &tmap_b, full_bar(stage), n_blk * BLOCK_N + i * 64, kb * kBlockK, img);
         } else {
           tma_load_2d(sb, &tmap_b, full_bar(stage), kb * kBlockK, n_blk * BLOCK_N);
+        }
+        if constexpr (STAGED) {
+          // the residual tile, right behind the first k-block: its latency hides under the mainloop.  Boxes wholly
+          // past M or N are not loaded (the tile exists, so box (0, 0) always is).
+          if (kb == 0 && p.has_res) {
+            constexpr int kCols = staged_chunk_cols<OutT>(), kChunks = BLOCK_N / kCols;
+            const int row0 = m_blk * kBlockM, col0 = n_blk * BLOCK_N;
+            const int rows = p.M - row0 > 64 ? 2 : 1, chunks = min(kChunks, (p.N - col0 + kCols - 1) / kCols);
+            mbar_expect_tx(res_bar, (uint32_t)(rows * chunks * kStagedBoxBytes));
+            for (int h = 0; h < rows; ++h)
+              for (int ch = 0; ch < chunks; ++ch)
+                tma_load_2d(smem_out + (uint32_t)((h * kChunks + ch) * kStagedBoxBytes), &tmap_r, res_bar,
+                            col0 + ch * kCols, row0 + 64 * h);
+          }
         }
         if (++stage == kStages) { stage = 0; phase ^= 1u; }
       }
@@ -257,6 +299,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     // ------------------------------- consumers -------------------------------
     const int wg = warp_idx >> 2;   // warpgroup: tile rows 64 wg .. 64 wg + 63
     const bool releaser = (threadIdx.x & 127) == 0;
+    if constexpr (STAGED) {
+      // the tile's bias and gamma, once: the load's latency overlaps the first k-block's TMA; read after a barrier in
+      // epilogue_staged.  Columns past N get neutral values (the store clips them anyway).
+      const int t = threadIdx.x, n = n_blk * BLOCK_N + (t % BLOCK_N);
+      if (t < BLOCK_N && p.bias != nullptr) s_bias[t] = n < p.N ? __ldg(p.bias + n) : 0.f;
+      if (t >= BLOCK_N && t < 2 * BLOCK_N && p.gamma != nullptr) s_gamma[t - BLOCK_N] = n < p.N ? __ldg(p.gamma + n) : 1.f;
+    }
     float acc[BLOCK_N / 2];
 #pragma unroll
     for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
@@ -289,6 +338,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     if (releaser) mbar_arrive(empty_bar(prev));
     if constexpr (MODE == kModeToken) epilogue_token<OutT, BLOCK_N>(p, acc, img, m_blk, n_blk, wg * 64);
     else if constexpr (MODE == kModeGluCols) epilogue_glu_cols<OutT, BLOCK_N>(p, acc, m_blk, n_blk, wg * 64);
+    else if constexpr (STAGED)
+      epilogue_staged<OutT, BLOCK_N>(p, acc, m_blk, n_blk, wg, smem_out, s_bias, s_gamma, res_bar, &tmap_c);
     else epilogue_frag<OutT, BLOCK_N>(p, acc, m_blk, n_blk, wg * 64);
   }
 }
@@ -305,16 +356,17 @@ int check_out(const void* C, long ldc, const void* residual, long ldr, int esize
 
 // Every launch of a gemm_wgmma_kernel instance: the shared-memory attribute, one CTA per 128 x BLOCK_N output tile (per
 // image for token mixing), the launch and its error check.
-template <int BLOCK_N, typename OutT, int AX, int MODE>
+// tc / tr: output and residual maps of the STAGED instances (unused otherwise).
+template <int BLOCK_N, typename OutT, int AX, int MODE, bool STAGED = false>
 int launch_wgmma(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, const char* what,
-                 cudaStream_t stream) {
-  using Cfg = GemmCfg<BLOCK_N>;
-  auto kernel = gemm_wgmma_kernel<BLOCK_N, OutT, AX, MODE>;
+                 cudaStream_t stream, const CUtensorMap& tc = CUtensorMap{}, const CUtensorMap& tr = CUtensorMap{}) {
+  using Cfg = GemmCfg<BLOCK_N, OutT, STAGED>;
+  auto kernel = gemm_wgmma_kernel<BLOCK_N, OutT, AX, MODE, STAGED>;
   static std::atomic<unsigned long long> attr_devs{0};  // per instantiation
   TFIMM_CUDA_OK(set_max_dynamic_smem(kernel, Cfg::kSmemBytes, attr_devs));
   const long imgs = MODE == kModeToken ? p.tk_imgs : 1;
   const long tiles = imgs * ((p.M + kBlockM - 1) / kBlockM) * ((p.N + BLOCK_N - 1) / BLOCK_N);
-  kernel<<<(unsigned)tiles, gemm_threads<BLOCK_N, AX>(), Cfg::kSmemBytes, stream>>>(ta, tb, p);
+  kernel<<<(unsigned)tiles, gemm_threads<BLOCK_N, AX>(), Cfg::kSmemBytes, stream>>>(ta, tb, tc, tr, p);
   TFIMM_LAUNCH_OK(what);
   return kOk;
 }
@@ -343,6 +395,22 @@ int launch_gemm(const void* A, int lda, const void* W, int ldw, const void* resi
   if ((st = make_tmap_2d(&ta, A, dtype_code<AX>(), M, K, lda, kBlockM, kBlockK, "A")) != kOk) return st;
   if ((st = make_tmap_2d(&tb, W, dtype_code<AX>(), N, K, ldw, BLOCK_N, kBlockK, "W")) != kOk) return st;
   p.c = C; p.res = residual; p.ldc = ldc; p.ldr = ldr;
+  // The plain bf16 GEMM at 64 / 128 columns stages its epilogue through shared memory (epilogue_staged).  The output
+  // and residual maps have the real extents (N, M) and their own row strides, in 64-row boxes of one 128-byte span.
+  // The TMA store clips a row only at a 16-byte boundary: with N * sizeof(OutT) % 16 != 0 (bf16 out, N % 8 != 0) it
+  // would overwrite the elements after column N up to that boundary, so those shapes keep the fragment epilogue.
+  constexpr bool kStaged = AX == kANone && MODE == kModeGemm && BLOCK_N <= 128;
+  if constexpr (kStaged) {
+    if ((long)N * (long)sizeof(OutT) % 16 != 0)
+      return launch_wgmma<BLOCK_N, OutT, AX, MODE>(ta, tb, p, "gemm_wgmma_kernel (bf16)", stream);
+    constexpr int es = (int)sizeof(OutT), dt = es == 2 ? kBF16 : kF32;
+    CUtensorMap tc, tr{};
+    if ((st = make_tmap_2d(&tc, C, dt, M, N, ldc, 64, staged_chunk_cols<OutT>(), "C")) != kOk) return st;
+    if (residual != nullptr &&
+        (st = make_tmap_2d(&tr, residual, dt, M, N, ldr, 64, staged_chunk_cols<OutT>(), "residual")) != kOk)
+      return st;
+    return launch_wgmma<BLOCK_N, OutT, AX, MODE, true>(ta, tb, p, "gemm_wgmma_kernel (bf16)", stream, tc, tr);
+  }
   return launch_wgmma<BLOCK_N, OutT, AX, MODE>(
       ta, tb, p,
       AX == kATf32 ? "gemm_wgmma_kernel (tf32)"
@@ -420,6 +488,9 @@ int pick_block_n(int M, int N) {
 //     ~ 128 * (K + kEpilogueK).
 //   BLOCK_N = 64, two CTAs per SM: one CTA's epilogue runs under the other's mainloop, so a wave of two tiles per SM
 //     costs ~ kPairWidth * K.
+// The constants were fitted with the fragment epilogue.  With the staged one, 128 ties 64 at the bias-only K = 768 ViT-B
+// shapes, loses to it by 10-15 % with the GELU epilogue (fc1) and wins by 20-25 % at K = 3072 (fc2): the choices this
+// model makes at those shapes, so it is kept until shapes where it chooses wrongly are measured.
 // BLOCK_N = 256 is not chosen: it was the slowest width at every measured shape (force_block_n still selects it).
 int pick_block_n_bf16(int M, int N, int K) {
   constexpr double kEpilogueK = 926.0, kPairWidth = 184.0;
