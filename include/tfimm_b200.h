@@ -58,7 +58,8 @@ int tfimm_b200_sm_count(void);
  * convnext.py:356-360, efficientnet.py:259-263) and 1x1 Conv2D (efficientnet_blocks.py:412-434,
  * resnet.py:220-248); gamma/residual fuse ConvNeXtBlock's layer-scale + shortcut (convnext.py:226-227).
  * force_block_n: 0 = auto; 64/128/256 = that tile width (testing / A-B measurements); 2 = the widest tile,
- * the same as 256. */
+ * the same as 256; 1 = the persistent kernel (128 x 256 tiles, one CTA per SM; bf16 output with N % 8 != 0 runs the
+ * 256-wide tile instead). */
 int tfimm_b200_gemm_bf16(const void* A, int lda, const void* W, int ldw, const float* bias,
                          const float* gamma, const void* residual, int ldr, void* C, int ldc, int M, int N,
                          int K, int act, int act_after_residual, int out_dtype, int force_block_n, void* stream);

@@ -229,34 +229,29 @@ __device__ __forceinline__ void st_staged_pair(__nv_bfloat16*, uint32_t a, uint6
   asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(pack_bf16x2(x, y)) : "memory");
 }
 
-// Epilogue of one warpgroup (rows 64 wg .. 64 wg + 63 of tile (m_blk, n_blk)) through the staged tile s_out.  The
-// per-element fp32 operations are those of epilogue_frag, in the same order.  s_bias / s_gamma hold the tile's BN
-// bias and gamma values, written by the consumer threads before their mainloop; res_bar completes when the residual
-// tile has landed in s_out (p.has_res).  Each element is read from and written back to s_out by the same thread, so
-// the residual may alias C: the TMA store of the tile is issued only after its residual load has completed.  The
-// output tensor map has the real extents (N, M), so the store clips the M and N tails.
-template <typename OutT, int BN>
-__device__ __forceinline__ void epilogue_staged(const GemmParams& p, float (&acc)[BN / 2], int m_blk, int n_blk, int wg,
-                                                uint32_t s_out, const float* s_bias, const float* s_gamma,
-                                                uint32_t res_bar, const CUtensorMap* tmap_c) {
-  constexpr int kCols = staged_chunk_cols<OutT>(), kChunks = BN / kCols;
+// Tile columns kFirst .. kFirst + kSpan - 1 of one warpgroup's accumulator, through its staged boxes at s_wg (tile
+// column kFirst is column 0 of the first box).  The per-element fp32 operations are those of epilogue_frag, in the
+// same order.  s_bias / s_gamma hold the tile's bias and gamma values; when the tile has a residual, it has landed in
+// the boxes.  Each element is read from and written back to the boxes by the same thread.
+// kAct >= 0: the activation, known at compile time; kAct < 0: p.act, chosen per column group at run time.
+template <typename OutT, int BN, int kFirst, int kSpan, int kAct>
+__device__ __forceinline__ void staged_apply_act(const GemmParams& p, float (&acc)[BN / 2], uint32_t s_wg,
+                                                 const float* s_bias, const float* s_gamma) {
+  const int act = kAct >= 0 ? kAct : p.act;
   const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3;
   const int r = wq * 16 + (lane >> 2);   // warpgroup row; r + 8 has the same swizzle phase
-  const uint32_t s_wg = s_out + (uint32_t)(wg * kChunks * kStagedBoxBytes);
   OutT* const tag = nullptr;
-  named_bar_sync<1>(256);   // s_bias / s_gamma were written by both consumer warpgroups
-  if (p.has_res) mbar_wait(res_bar, 0);
 #pragma unroll
-  for (int g = 0; g < BN / 8; ++g) {
+  for (int g = kFirst / 8; g < (kFirst + kSpan) / 8; ++g) {
     const int c = g * 8 + 2 * (lane & 3);
-    const uint32_t a0 = staged_addr<OutT>(s_wg, r, c), a1 = a0 + 8 * 128;
+    const uint32_t a0 = staged_addr<OutT>(s_wg, r, c - kFirst), a1 = a0 + 8 * 128;
     uint64_t v[2] = {pack2(acc[4 * g + 0], acc[4 * g + 1]), pack2(acc[4 * g + 2], acc[4 * g + 3])};
     if (p.bias != nullptr) {
       const float2 b = *reinterpret_cast<const float2*>(s_bias + c);
       v[0] = add2(v[0], pack2(b.x, b.y));
       v[1] = add2(v[1], pack2(b.x, b.y));
     }
-    if (!p.act_post) apply_act_pairs(v, p.act);
+    if (!p.act_post) apply_act_pairs(v, act);
     if (p.gamma != nullptr) {
       const float2 s = *reinterpret_cast<const float2*>(s_gamma + c);
       v[0] = mul2(v[0], pack2(s.x, s.y));
@@ -266,22 +261,63 @@ __device__ __forceinline__ void epilogue_staged(const GemmParams& p, float (&acc
       v[0] = add2(v[0], ld_staged_pair(tag, a0));
       v[1] = add2(v[1], ld_staged_pair(tag, a1));
     }
-    if (p.act_post) apply_act_pairs(v, p.act);
+    if (p.act_post) apply_act_pairs(v, act);
     st_staged_pair(tag, a0, v[0]);
     st_staged_pair(tag, a1, v[1]);
   }
-  // generic-proxy writes -> visible to the TMA engine, then one thread stores the warpgroup's rows
-  fence_proxy_async_smem();
+}
+
+// The common activations are dispatched once here rather than in every column group.  Unrolled over the groups, a
+// per-group switch inlines every activation's code into each group; the epilogue's code then outgrows the instruction
+// cache, and the jumps over the untaken cases make every tile's epilogue fetch it again.
+template <typename OutT, int BN, int kFirst, int kSpan>
+__device__ __forceinline__ void staged_apply(const GemmParams& p, float (&acc)[BN / 2], uint32_t s_wg,
+                                             const float* s_bias, const float* s_gamma) {
+  switch (p.act) {
+    case kActNone: staged_apply_act<OutT, BN, kFirst, kSpan, kActNone>(p, acc, s_wg, s_bias, s_gamma); break;
+    case kActGelu: staged_apply_act<OutT, BN, kFirst, kSpan, kActGelu>(p, acc, s_wg, s_bias, s_gamma); break;
+    case kActSwish: staged_apply_act<OutT, BN, kFirst, kSpan, kActSwish>(p, acc, s_wg, s_bias, s_gamma); break;
+    default: staged_apply_act<OutT, BN, kFirst, kSpan, -1>(p, acc, s_wg, s_bias, s_gamma); break;
+  }
+}
+
+// Barrier over the 128 threads of consumer warpgroup wg.
+__device__ __forceinline__ void warpgroup_bar_sync(int wg) {
   if (wg == 0) named_bar_sync<2>(128);
   else named_bar_sync<3>(128);
+}
+
+// One thread's TMA store of up to kChunks staged boxes of a warpgroup (rows row0 .., columns col0 ..), then the commit.
+// Boxes wholly past N are not stored; the tensor map's extents clip the rest.
+template <typename OutT, int kChunks>
+__device__ __forceinline__ void staged_store(const GemmParams& p, const CUtensorMap* tmap_c, uint32_t s_wg, int row0,
+                                             int col0) {
+  constexpr int kCols = staged_chunk_cols<OutT>();
+#pragma unroll
+  for (int ch = 0; ch < kChunks; ++ch)
+    if (col0 + ch * kCols < p.N) tma_store_2d(tmap_c, s_wg + (uint32_t)(ch * kStagedBoxBytes), col0 + ch * kCols, row0);
+  tma_store_commit();
+}
+
+// Epilogue of one warpgroup (rows 64 wg .. 64 wg + 63 of tile (m_blk, n_blk)) through the staged tile s_out.  s_bias /
+// s_gamma were written by the consumer threads before their mainloop; res_bar completes when the residual tile has
+// landed in s_out (p.has_res).  The residual may alias C: the TMA store of the tile is issued only after its residual
+// load has completed.  The output tensor map has the real extents (N, M), so the store clips the M and N tails.
+template <typename OutT, int BN>
+__device__ __forceinline__ void epilogue_staged(const GemmParams& p, float (&acc)[BN / 2], int m_blk, int n_blk, int wg,
+                                                uint32_t s_out, const float* s_bias, const float* s_gamma,
+                                                uint32_t res_bar, const CUtensorMap* tmap_c) {
+  constexpr int kChunks = BN / staged_chunk_cols<OutT>();
+  const uint32_t s_wg = s_out + (uint32_t)(wg * kChunks * kStagedBoxBytes);
+  named_bar_sync<1>(256);   // s_bias / s_gamma were written by both consumer warpgroups
+  if (p.has_res) mbar_wait(res_bar, 0);
+  staged_apply<OutT, BN, 0, BN>(p, acc, s_wg, s_bias, s_gamma);
+  // generic-proxy writes -> visible to the TMA engine, then one thread stores the warpgroup's rows
+  fence_proxy_async_smem();
+  warpgroup_bar_sync(wg);
   const int row0 = m_blk * 128 + wg * 64;
   if ((threadIdx.x & 127) == 0 && row0 < p.M) {
-#pragma unroll
-    for (int ch = 0; ch < kChunks; ++ch) {
-      const int col0 = n_blk * BN + ch * kCols;
-      if (col0 < p.N) tma_store_2d(tmap_c, s_wg + (uint32_t)(ch * kStagedBoxBytes), col0, row0);
-    }
-    tma_store_commit();
+    staged_store<OutT, kChunks>(p, tmap_c, s_wg, row0, n_blk * BN);
     tma_store_wait_read<0>();   // the tile must not be released before the TMA engine has read it
   }
 }

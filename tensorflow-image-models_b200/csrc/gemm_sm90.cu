@@ -19,6 +19,8 @@
 //   warps 9..12 (A-transform instances only) rewrite the A tile in smem before the MMA reads it: the squeeze-excite
 //               gate (bf16), or the TF32 rounding of fp32 activations (precision="tf32")
 //
+// gemm_persistent_kernel is the plain bf16 GEMM at 128 x 256 tiles with one CTA per SM walking the tiles (see there).
+//
 // Two more instances share the ring, barriers, producer/consumer split and epilogue plumbing (GemmMode):
 //   kModeToken   token mixing, out[b][m][c] = epi(sum_n Wt[m][n] X[b][n][c]): the Dense layer that MLP-Mixer, ResMLP
 //                and gMLP apply along the token axis of a transposed activation.  B is X where it is stored, read
@@ -344,6 +346,176 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   }
 }
 
+// ---------------------- persistent 128 x 256 instance ----------------------
+// The plain bf16 GEMM with the staged epilogue, one CTA per SM: CTA c takes tiles c, c + gridDim.x, ... in the n-fastest
+// order of the per-tile grid.  A 128 x 256 tile loads half the operand bytes per MAC of a 128 x 64 one.  The producer's
+// ring stage and phase run on across tiles, so it fills the next tile's first k-blocks while the consumers run the
+// epilogue, and the tensor cores restart on a full ring.
+// Shared memory: 3 stages of 48 KB, a 64 KB staging buffer of four 8 KB boxes per warpgroup (the whole bf16 tile, or
+// one 128-column half of the fp32 tile), bias and gamma of two tiles (one warpgroup may still read tile i's while the
+// other writes tile i + 1's), and the barriers: 213 KB.
+struct PersistentCfg {
+  static constexpr int kBlockN = 256;
+  static constexpr int kABytes = kBlockM * kRowBytes;
+  static constexpr int kStageBytes = kABytes + kBlockN * kRowBytes;
+  static constexpr int kStages = 3;
+  static constexpr int kBoxes = 4;   // staged boxes per warpgroup
+  static constexpr int kOutBytes = 2 * kBoxes * kStagedBoxBytes;
+  static constexpr int kVecBytes = 2 * 2 * kBlockN * 4;
+  static constexpr int kNumBarriers = 2 * kStages + 2;   // full, empty, one residual barrier per warpgroup
+  static constexpr int kSmemBytes = kStages * kStageBytes + kOutBytes + kVecBytes + kNumBarriers * 8 + 1024;
+};
+
+// Each warpgroup's leader thread (its thread 0) moves the warpgroup's staged rows: it loads the residual span into them
+// by TMA and stores the result from them.  Before the next residual load or epilogue reuses the boxes, it waits until
+// the previous store has read them (cp.async.bulk.wait_group.read); for a tile's first span that wait and the residual
+// load are issued right after the tile's first k-block, so both hide under the mainloop.  fp32 output takes two spans of
+// 128 columns: the second span's residual is loaded once the first span's store has been read out.  In place is safe:
+// tiles are disjoint, and a span is stored after its own residual has landed.
+template <typename OutT>
+__global__ void __launch_bounds__(kConsumerThreads + 32, 1)
+gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                       const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ CUtensorMap tmap_r,
+                       const GemmParams p) {
+  using Cfg = PersistentCfg;
+  constexpr int BN = Cfg::kBlockN, kStages = Cfg::kStages, kBlockK = 64;
+  constexpr int kCols = staged_chunk_cols<OutT>(), kSpan = Cfg::kBoxes * kCols;   // 256 bf16 / 128 fp32 columns
+
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_tiles = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t smem_out = smem_tiles + kStages * Cfg::kStageBytes;
+  const uint32_t smem_vec = smem_out + Cfg::kOutBytes;
+  const uint32_t smem_bars = smem_vec + Cfg::kVecBytes;
+  auto full_bar = [&](int s) { return smem_bars + 8u * s; };
+  auto empty_bar = [&](int s) { return smem_bars + 8u * (kStages + s); };
+  float* const s_vec = reinterpret_cast<float*>(smem_raw + (smem_vec - smem_u32(smem_raw)));
+
+  const int warp_idx = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  if (warp_idx == kProducerWarp && lane == 0) {
+    prefetch_tmap(&tmap_a);
+    prefetch_tmap(&tmap_b);
+    prefetch_tmap(&tmap_c);
+    if (p.has_res) prefetch_tmap(&tmap_r);
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(full_bar(s), 1);
+      mbar_init(empty_bar(s), 2);   // one arrival per consumer warpgroup
+    }
+    mbar_init(smem_bars + 8u * (2 * kStages), 1);
+    mbar_init(smem_bars + 8u * (2 * kStages + 1), 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  const int num_n_tiles = (p.N + BN - 1) / BN;
+  const int tiles = ((p.M + kBlockM - 1) / kBlockM) * num_n_tiles;
+  const int num_k_blocks = (p.K + kBlockK - 1) / kBlockK;
+
+  if (warp_idx == kProducerWarp) {
+    // ------------------------------ TMA producer ------------------------------
+    if (threadIdx.x == kProducerWarp * 32) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+        const int m_blk = t / num_n_tiles, n_blk = t % num_n_tiles;
+        for (int kb = 0; kb < num_k_blocks; ++kb) {
+          mbar_wait(empty_bar(stage), phase ^ 1u);
+          const uint32_t sa = smem_tiles + stage * Cfg::kStageBytes;
+          mbar_expect_tx(full_bar(stage), Cfg::kStageBytes);
+          tma_load_2d(sa, &tmap_a, full_bar(stage), kb * kBlockK, m_blk * kBlockM);
+          tma_load_2d(sa + Cfg::kABytes, &tmap_b, full_bar(stage), kb * kBlockK, n_blk * BN);
+          if (++stage == kStages) { stage = 0; phase ^= 1u; }
+        }
+      }
+    }
+    return;
+  }
+
+  // ------------------------------- consumers -------------------------------
+  const int wg = warp_idx >> 2;   // warpgroup: tile rows 64 wg .. 64 wg + 63
+  const bool leader = (threadIdx.x & 127) == 0;
+  const uint32_t s_wg = smem_out + (uint32_t)(wg * Cfg::kBoxes * kStagedBoxBytes);
+  const uint32_t res_bar = smem_bars + 8u * (2 * kStages + wg);
+  int stage = 0, prev = 0, buf = 0;
+  uint32_t phase = 0, res_phase = 0;
+  for (int t = blockIdx.x; t < tiles; t += gridDim.x, buf ^= 1) {
+    const int m_blk = t / num_n_tiles, n_blk = t % num_n_tiles;
+    const int row0 = m_blk * kBlockM + wg * 64;
+    // span h of this warpgroup's rows has a residual to load (uniform over the warpgroup)
+    auto has_res_span = [&](int h) { return p.has_res && row0 < p.M && n_blk * BN + h * kSpan < p.N; };
+    auto load_res_span = [&](int h) {   // leader only
+      const int col0 = n_blk * BN + h * kSpan, chunks = min(Cfg::kBoxes, (p.N - col0 + kCols - 1) / kCols);
+      mbar_expect_tx(res_bar, (uint32_t)(chunks * kStagedBoxBytes));
+      for (int ch = 0; ch < chunks; ++ch)
+        tma_load_2d(s_wg + (uint32_t)(ch * kStagedBoxBytes), &tmap_r, res_bar, col0 + ch * kCols, row0);
+    };
+    // the tile's bias and gamma (columns past N get neutral values): loaded here, written to shared memory once the
+    // first k-block's MMAs are issued, so the load's latency does not delay them; read after a barrier in the epilogue
+    float* const s_bias = s_vec + buf * 2 * BN;
+    float* const s_gamma = s_bias + BN;
+    const int n_own = n_blk * BN + threadIdx.x;
+    const float bias_own = p.bias != nullptr && n_own < p.N ? __ldg(p.bias + n_own) : 0.f;
+    const float gamma_own = p.gamma != nullptr && n_own < p.N ? __ldg(p.gamma + n_own) : 1.f;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int kb = 0; kb < num_k_blocks; ++kb) {
+      mbar_wait(full_bar(stage), phase);
+      const uint32_t sa = smem_tiles + stage * Cfg::kStageBytes;
+      const uint64_t da = gmma_desc_k_sw128(sa + (uint32_t)wg * (64 * 128));
+      const uint64_t db = gmma_desc_k_sw128(sa + Cfg::kABytes);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_ss<BN, false>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (uint32_t)((kb | k) != 0));
+      wgmma_commit();
+      if (kb == 0) {
+        s_bias[threadIdx.x] = bias_own;
+        s_gamma[threadIdx.x] = gamma_own;
+      }
+      // halfway through the mainloop, the previous tile's store has long read the staged boxes: the leader's wait
+      // (which holds up its warpgroup's next MMAs) is short, and the residual has the other half to land
+      if (kb == num_k_blocks / 2 && leader) {
+        tma_store_wait_read<0>();
+        if (has_res_span(0)) load_res_span(0);
+      }
+      wgmma_wait<1>();
+      if (kb > 0 && leader) mbar_arrive(empty_bar(prev));
+      prev = stage;
+      if (++stage == kStages) { stage = 0; phase ^= 1u; }
+    }
+    wgmma_wait<0>();
+    if (leader) mbar_arrive(empty_bar(prev));
+
+    // ------------------------------- epilogue -------------------------------
+    named_bar_sync<1>(256);   // s_bias / s_gamma were written by both consumer warpgroups
+    auto span = [&](auto h_const) {
+      constexpr int h = decltype(h_const)::value;
+      if (n_blk * BN + h * kSpan >= p.N) return;
+      if constexpr (h > 0) {
+        // the boxes hold the previous span until its store has read them
+        if (leader) {
+          tma_store_wait_read<0>();
+          if (has_res_span(h)) load_res_span(h);
+        }
+        warpgroup_bar_sync(wg);
+      }
+      if (has_res_span(h)) {
+        mbar_wait(res_bar, res_phase);
+        res_phase ^= 1u;
+      }
+      staged_apply<OutT, BN, h * kSpan, kSpan>(p, acc, s_wg, s_bias, s_gamma);
+      // generic-proxy writes -> visible to the TMA engine, then the leader stores the span
+      fence_proxy_async_smem();
+      warpgroup_bar_sync(wg);
+      if (leader && row0 < p.M) staged_store<OutT, Cfg::kBoxes>(p, &tmap_c, s_wg, row0, n_blk * BN + h * kSpan);
+    };
+    span(std::integral_constant<int, 0>{});
+    if constexpr (kSpan < BN) span(std::integral_constant<int, 1>{});
+  }
+  if (leader) tma_store_wait_read<0>();   // the CTA's shared memory must outlive the last store's reads
+}
+
 // ------------------------------ host side -----------------------------------
 // Output / residual: 16-byte aligned base and row stride (vector epilogue accesses, as the layout of every caller).
 int check_out(const void* C, long ldc, const void* residual, long ldr, int esize) {
@@ -384,9 +556,27 @@ int with_block_n(int bn, const char* unsupported_fmt, F&& launch) {
   return kInvalidArgument;
 }
 
-template <int BLOCK_N, typename OutT, int AX = kANone, int MODE = kModeGemm>
+// The persistent 128 x 256 instance: one CTA per SM, or one per tile when there are fewer tiles.
+template <typename OutT>
+int launch_persistent(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, const CUtensorMap& tr,
+                      const GemmParams& p, cudaStream_t stream) {
+  using Cfg = PersistentCfg;
+  auto kernel = gemm_persistent_kernel<OutT>;
+  static std::atomic<unsigned long long> attr_devs{0};  // per instantiation
+  TFIMM_CUDA_OK(set_max_dynamic_smem(kernel, Cfg::kSmemBytes, attr_devs));
+  const long tiles = (long)((p.M + kBlockM - 1) / kBlockM) * ((p.N + Cfg::kBlockN - 1) / Cfg::kBlockN);
+  const int grid = (int)std::min<long>(tiles, sm_count());
+  kernel<<<grid, kConsumerThreads + 32, Cfg::kSmemBytes, stream>>>(ta, tb, tc, tr, p);
+  TFIMM_LAUNCH_OK("gemm_persistent_kernel (bf16)");
+  return kOk;
+}
+
+// PERSISTENT (BLOCK_N = 256, plain bf16 GEMM): the persistent instance instead of the per-tile one.
+template <int BLOCK_N, typename OutT, int AX = kANone, int MODE = kModeGemm, bool PERSISTENT = false>
 int launch_gemm(const void* A, int lda, const void* W, int ldw, const void* residual, int ldr, void* C, int ldc,
                 GemmParams p, cudaStream_t stream) {
+  static_assert(!PERSISTENT || (BLOCK_N == PersistentCfg::kBlockN && AX == kANone && MODE == kModeGemm),
+                "the persistent instance is the plain bf16 GEMM at 256 columns");
   const int M = p.M, N = p.N, K = p.K;
   constexpr int kBlockK = block_k<AX>();
   CUtensorMap ta, tb;
@@ -395,11 +585,11 @@ int launch_gemm(const void* A, int lda, const void* W, int ldw, const void* resi
   if ((st = make_tmap_2d(&ta, A, dtype_code<AX>(), M, K, lda, kBlockM, kBlockK, "A")) != kOk) return st;
   if ((st = make_tmap_2d(&tb, W, dtype_code<AX>(), N, K, ldw, BLOCK_N, kBlockK, "W")) != kOk) return st;
   p.c = C; p.res = residual; p.ldc = ldc; p.ldr = ldr;
-  // The plain bf16 GEMM at 64 / 128 columns stages its epilogue through shared memory (epilogue_staged).  The output
-  // and residual maps have the real extents (N, M) and their own row strides, in 64-row boxes of one 128-byte span.
-  // The TMA store clips a row only at a 16-byte boundary: with N * sizeof(OutT) % 16 != 0 (bf16 out, N % 8 != 0) it
-  // would overwrite the elements after column N up to that boundary, so those shapes keep the fragment epilogue.
-  constexpr bool kStaged = AX == kANone && MODE == kModeGemm && BLOCK_N <= 128;
+  // The plain bf16 GEMM at 64 / 128 columns and the persistent instance stage their epilogue through shared memory.  The
+  // output and residual maps have the real extents (N, M) and their own row strides, in 64-row boxes of one 128-byte
+  // span.  The TMA store clips a row only at a 16-byte boundary: with N * sizeof(OutT) % 16 != 0 (bf16 out, N % 8 != 0)
+  // it would overwrite the elements after column N up to that boundary, so those shapes keep the fragment epilogue.
+  constexpr bool kStaged = AX == kANone && MODE == kModeGemm && (BLOCK_N <= 128 || PERSISTENT);
   if constexpr (kStaged) {
     if ((long)N * (long)sizeof(OutT) % 16 != 0)
       return launch_wgmma<BLOCK_N, OutT, AX, MODE>(ta, tb, p, "gemm_wgmma_kernel (bf16)", stream);
@@ -409,7 +599,8 @@ int launch_gemm(const void* A, int lda, const void* W, int ldw, const void* resi
     if (residual != nullptr &&
         (st = make_tmap_2d(&tr, residual, dt, M, N, ldr, 64, staged_chunk_cols<OutT>(), "residual")) != kOk)
       return st;
-    return launch_wgmma<BLOCK_N, OutT, AX, MODE, true>(ta, tb, p, "gemm_wgmma_kernel (bf16)", stream, tc, tr);
+    if constexpr (PERSISTENT) return launch_persistent<OutT>(ta, tb, tc, tr, p, stream);
+    else return launch_wgmma<BLOCK_N, OutT, AX, MODE, true>(ta, tb, p, "gemm_wgmma_kernel (bf16)", stream, tc, tr);
   }
   return launch_wgmma<BLOCK_N, OutT, AX, MODE>(
       ta, tb, p,
@@ -481,9 +672,14 @@ int pick_block_n(int M, int N) {
   return best;
 }
 
-// Tile width of the plain bf16 GEMM (tfimm_b200_gemm_bf16), from its wave count and a per-wave time fitted to
-// measurements of that kernel (profiles/gemm_h100.md).  The other instances keep pick_block_n: their kernels (A-transform
-// warps, TF32 k-blocks, token mixing) were not measured against this model.
+// Tile width of the plain bf16 GEMM (tfimm_b200_gemm_bf16), fitted to measurements of its kernels (profiles/gemm_h100.md).
+// The other instances keep pick_block_n: their kernels (A-transform warps, TF32 k-blocks, token mixing) were not measured
+// against this rule.
+// The persistent 128 x 256 instance, when its TMA store applies (not bf16 output with N % 8 != 0), its tiles fill every
+// SM, and N > 256.  It measured fastest at every ViT-B, ConvNeXt-B and Swin-B shape with more than 256 columns, by
+// 10-40 %, down to K = 128.  At N <= 256 (Swin-B's stage 1 and 2 proj: fp32 residual, bound by HBM) it was 2-8 % slower
+// than the 64-wide tile; with N = 128 half of each 256-wide tile is empty.  Below one tile per SM it was not measured.
+// Otherwise, from a wave count and a per-wave time:
 //   BLOCK_N = 128, one CTA per SM: the epilogue runs after the mainloop with the tensor cores idle, so a wave costs
 //     ~ 128 * (K + kEpilogueK).
 //   BLOCK_N = 64, two CTAs per SM: one CTA's epilogue runs under the other's mainloop, so a wave of two tiles per SM
@@ -491,11 +687,15 @@ int pick_block_n(int M, int N) {
 // The constants were fitted with the fragment epilogue.  With the staged one, 128 ties 64 at the bias-only K = 768 ViT-B
 // shapes, loses to it by 10-15 % with the GELU epilogue (fc1) and wins by 20-25 % at K = 3072 (fc2): the choices this
 // model makes at those shapes, so it is kept until shapes where it chooses wrongly are measured.
-// BLOCK_N = 256 is not chosen: it was the slowest width at every measured shape (force_block_n still selects it).
-int pick_block_n_bf16(int M, int N, int K) {
+// The per-tile BLOCK_N = 256 instance is not chosen: it was the slowest width at every measured shape (force_block_n
+// still selects it).
+constexpr int kPersistent = 1;   // force_block_n / pick_block_n_bf16 value of the persistent 128 x 256 instance
+
+int pick_block_n_bf16(int M, int N, int K, int out_dtype) {
   constexpr double kEpilogueK = 926.0, kPairWidth = 184.0;
   const int sms = sm_count() > 0 ? sm_count() : 132;  // no device (host-side shape queries): H100 SXM
   const long mt = (M + kBlockM - 1) / kBlockM;
+  if (N > 256 && (out_dtype == kF32 || N % 8 == 0) && mt * ((N + 255) / 256) >= sms) return kPersistent;
   const long waves128 = (mt * ((N + 127) / 128) + sms - 1) / sms;
   const long waves64 = (mt * ((N + 63) / 64) + 2 * sms - 1) / (2 * sms);
   return (double)waves64 * kPairWidth * K < (double)waves128 * 128.0 * (K + kEpilogueK) ? 64 : 128;
@@ -557,8 +757,13 @@ int tfimm_b200_gemm_bf16(const void* A, int lda, const void* W, int ldw, const f
   GemmParams p{};
   p.M = M; p.N = N; p.K = K;
   p.bias = bias; p.gamma = gamma; p.act = act; p.has_res = residual != nullptr ? 1 : 0; p.act_post = act_post;
-  // force_block_n: 0 = choose; 64/128/256 = that tile width; 2 = the widest tile (256)
-  const int bn = force_block_n == 2 ? 256 : (force_block_n > 0 ? force_block_n : pick_block_n_bf16(M, N, K));
+  // force_block_n: 0 = choose; 64/128/256 = that tile width; 2 = the widest tile (256); 1 = the persistent instance
+  const int bn =
+      force_block_n == 2 ? 256 : (force_block_n > 0 ? force_block_n : pick_block_n_bf16(M, N, K, out_dtype));
+  if (bn == kPersistent)
+    return out_dtype == kBF16
+               ? launch_gemm<256, __nv_bfloat16, kANone, kModeGemm, true>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream)
+               : launch_gemm<256, float, kANone, kModeGemm, true>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream);
   return with_block_n<256>(bn, "gemm: unsupported block_n %d", [&](auto n) {
     constexpr int BN = decltype(n)::value;
     return out_dtype == kBF16 ? launch_gemm<BN, __nv_bfloat16>(A, lda, W, ldw, residual, ldr, C, ldc, p, stream)

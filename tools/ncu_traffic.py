@@ -24,7 +24,7 @@ FAMILIES = [
     ("mlp_fused", "mlp_bf16"),
     # the TF32 instances of the wgmma GEMM (template argument A-transform = 2, fp32 out) before the bf16 ones
     ("gemm_wgmma_kernelILi64EfLi2E", "gemm_tf32"), ("gemm_wgmma_kernelILi128EfLi2E", "gemm_tf32"),
-    ("gemm_wgmma", "gemm_bf16"), ("gemm_bf16_skinny", "gemm_bf16"),
+    ("gemm_wgmma", "gemm_bf16"), ("gemm_persistent", "gemm_bf16"), ("gemm_bf16_skinny", "gemm_bf16"),
     # before "gemm_f32": the MLP-Mixer fp32 token-mixing kernel's name contains it
     ("token_gemm_f32", "token_gemm_f32"), ("affine_kernel", "affine"),
     ("gemm_f32", "gemm_f32"),
