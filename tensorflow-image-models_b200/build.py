@@ -46,7 +46,8 @@ def build(force: bool = False, verbose: bool = False, defines=(), out: Path = No
     if defines or out is not None:
         return _build_variant(list(defines), Path(out or (OBJ_DIR / "libtfimm_b200_variant.so")))
     sources = sorted(CSRC.glob("*.cu"))
-    headers = sorted(CSRC.glob("*.cuh")) + [ROOT.parent / "include" / "tfimm_b200.h"]
+    headers = sorted(CSRC.glob("*.cuh")) + [ROOT.parent / "include" / "tfimm_b200.h",
+                                            ROOT.parent / "include" / "tfimm_b200_poolformer.h"]
     stamp = OBJ_DIR / "stamp.txt"
     digest = _digest(sources + headers)
     if not force and LIB.exists() and stamp.exists() and stamp.read_text() == digest:

@@ -59,14 +59,15 @@ TRACE_FAMILY.update({
 })
 
 
-def _call(name, dev, *args, flops=0.0, nbytes=0.0):
+def _call(name, dev, *args, flops=0.0, nbytes=0.0, family=None):
     """Calls entry point ``name`` with ``args`` and the current stream of ``dev`` (every entry point takes its stream
-    last), with ``dev`` as the current device: cudaFuncSetAttribute, the launch and the SM count all refer to it."""
+    last), with ``dev`` as the current device: cudaFuncSetAttribute, the launch and the SM count all refer to it.
+    ``family``: the trace family of an entry point outside ``lib.SIGNATURES`` (the optional families' own tables)."""
     global launch_count
     fn = getattr(_lib.load(), name)
     if dev.index != torch.cuda.current_device():
         with torch.cuda.device(dev):
-            return _call(name, dev, *args, flops=flops, nbytes=nbytes)
+            return _call(name, dev, *args, flops=flops, nbytes=nbytes, family=family)
     args = (*args, torch.cuda.current_stream(dev).cuda_stream)
     if trace is not None:
         e0 = torch.cuda.Event(enable_timing=True)
@@ -74,7 +75,7 @@ def _call(name, dev, *args, flops=0.0, nbytes=0.0):
         e0.record()
         _lib.check(fn(*args), name)
         e1.record()
-        trace.append((TRACE_FAMILY[name], e0, e1, float(flops), float(nbytes)))
+        trace.append((family or TRACE_FAMILY[name], e0, e1, float(flops), float(nbytes)))
     else:
         _lib.check(fn(*args), name)
     launch_count += 1

@@ -20,7 +20,7 @@ from pathlib import Path
 
 REFERENCE = Path("/root/reference")
 OUT = Path(__file__).resolve().parent.parent / "tensorflow-image-models_b200" / "tfimm" / "architectures" / "zoo"
-FAMILIES = ["vit", "swin", "convnext", "efficientnet", "resnet", "mlp_mixer"]
+FAMILIES = ["vit", "swin", "convnext", "efficientnet", "resnet", "mlp_mixer", "poolformer"]
 
 
 class _Meta(type):

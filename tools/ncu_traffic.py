@@ -27,6 +27,7 @@ FAMILIES = [
     ("gemm_wgmma", "gemm_bf16"), ("gemm_persistent", "gemm_bf16"), ("gemm_bf16_skinny", "gemm_bf16"),
     # before "gemm_f32": the MLP-Mixer fp32 token-mixing kernel's name contains it
     ("token_gemm_f32", "token_gemm_f32"), ("affine_kernel", "affine"),
+    ("gn1_partials", "gn1_partials"), ("poolformer_mixer", "poolformer_mixer"), ("gn1_apply", "gn1_apply"),
     ("gemm_f32", "gemm_f32"),
     # before "attention_f32": the Segment Anything kernels' names contain it
     ("relpos_attention_bf16", "relpos_attention_bf16"), ("relpos_attention_f32", "relpos_attention_f32"),
