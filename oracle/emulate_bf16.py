@@ -146,18 +146,52 @@ def patch_merge_ln(x, gamma, beta, eps, out_dtype):
     return _ln(cat, gamma, beta, eps).reshape(-1, cat.shape[-1]).contiguous().to(out_dtype)
 
 
-def _softmax_pv(s, v, round_p):
-    """softmax(s) @ v the way the tensor-core kernels do it: p = exp(s - max) in fp32, the row sum of the fp32 p,
-    p rounded to bf16 for the PV product, fp32 accumulation, division by the row sum at the end."""
-    m = s.amax(dim=-1, keepdim=True)
-    p = torch.exp(s - m)
+# Keys per block of the online softmax of the tensor-core attention kernels (csrc/attention.cu, pit.cu,
+# relpos_attention.cu).
+KEY_BLOCK = 64
+
+
+def round_bf16(p):
+    """P as a bf16 tensor-core operand sees it: rounded to nearest even, kept in p's dtype."""
+    return p.to(torch.bfloat16).to(p.dtype)
+
+
+def _softmax_pv(s, v, round_p=None, key_block=None):
+    """softmax(s) @ v the way the tensor-core kernels do it: an online softmax over blocks of ``key_block`` keys from
+    key 0 (None: the whole row in one block).  Per block, m = the largest score so far, p = exp(s - m), the row sum
+    l = l exp(m_old - m) + sum p of the unrounded p, O = O exp(m_old - m) + round_p(p) V; O / l at the end.
+    ``round_p``: the rounding of P for the PV product (``round_bf16``, TF32, or None).  Also returns the normalised
+    (rounded) P when the row is one block, else None."""
+    N = s.shape[-1]
+    kb = N if key_block is None else key_block
+    rnd = round_p if round_p is not None else (lambda p: p)
+    m = s[..., :kb].amax(dim=-1, keepdim=True)
+    p = torch.exp(s[..., :kb] - m)
     l = p.sum(dim=-1, keepdim=True)
-    if round_p:
-        p = p.to(torch.bfloat16).to(_HP)
-    return (p @ v) / l, p / l
+    p = rnd(p)
+    o = p @ v[..., :kb, :]
+    for j0 in range(kb, N, kb):
+        sb = s[..., j0:j0 + kb]
+        m_new = torch.maximum(m, sb.amax(dim=-1, keepdim=True))
+        alpha = torch.exp(m - m_new)
+        pb = torch.exp(sb - m_new)
+        l = l * alpha + pb.sum(dim=-1, keepdim=True)
+        o = o * alpha + rnd(pb) @ v[..., j0:j0 + kb, :]
+        m = m_new
+    return o / l, (p / l if kb >= N else None)
 
 
-def attention(qkv, B, N, H, dh, scale, bias=None, mask=None, probs=None, row_map=None, nw_img=0):
+def image_chunks(B, H, N, budget=2 ** 24):
+    """Slices of the image axis whose (images, H, N, N) score tensors hold at most ``budget`` elements (at least one
+    image each): the float64 statements and bounds of attention are computed chunk by chunk, so that a benchmark batch
+    of ViT-B (256 x 12 x 197^2) does not hold its whole score tensor and its temporaries at once."""
+    step = max(1, budget // (H * N * N))
+    return [slice(b0, min(B, b0 + step)) for b0 in range(0, B, step)]
+
+
+def attention(qkv, B, N, H, dh, scale, bias=None, mask=None, probs=None, row_map=None, nw_img=0, key_block=KEY_BLOCK):
+    """bf16 qkv: P rounded to bf16 per block of ``key_block`` keys (the tensor-core kernels; the window kernels pass
+    None: one block); fp32 qkv: the SIMT kernel's unrounded softmax over the whole row."""
     dt = qkv.dtype
     x = qkv.to(_HP)
     if row_map is not None:  # Swin: rows of window w of image b live at row_map[w*N + i] of that image's tokens
@@ -166,15 +200,21 @@ def attention(qkv, B, N, H, dh, scale, bias=None, mask=None, probs=None, row_map
         idx = (torch.arange(nimg, device=x.device)[:, None] * tok + row_map.long()[None, :]).reshape(-1)
         x = x[idx]
     q, k, v = x.view(B, N, 3, H, dh).permute(2, 0, 3, 1, 4)
-    s = scale * (q @ k.transpose(-1, -2))
-    if bias is not None:
-        s = s + bias.to(_HP)[None]
-    if mask is not None:
-        nm = mask.shape[0]
-        s = (s.view(B // nm, nm, H, N, N) + mask.to(_HP)[None, :, None]).view(B, H, N, N)
-    o, p = _softmax_pv(s, v, round_p=(dt == torch.bfloat16))
-    if probs is not None:
-        probs.copy_(p)
+    round_p = round_bf16 if dt == torch.bfloat16 else None
+    if bias is None and mask is None and probs is None:
+        o = torch.cat([_softmax_pv(scale * (q[c] @ k[c].transpose(-1, -2)), v[c], round_p,
+                                   key_block if round_p is not None else None)[0]
+                       for c in image_chunks(B, H, N)])
+    else:
+        s = scale * (q @ k.transpose(-1, -2))
+        if bias is not None:
+            s = s + bias.to(_HP)[None]
+        if mask is not None:
+            nm = mask.shape[0]
+            s = (s.view(B // nm, nm, H, N, N) + mask.to(_HP)[None, :, None]).view(B, H, N, N)
+        o, p = _softmax_pv(s, v, round_p, key_block if round_p is not None else None)
+        if probs is not None:
+            probs.copy_(p)
     o = o.permute(0, 2, 1, 3).reshape(B * N, H * dh)
     if row_map is not None:
         out = torch.empty_like(o)
@@ -195,7 +235,8 @@ def window_attention(qkv, bias, row_map, labels, B, nw_img, N, H, dh, scale):
     if labels is not None:
         lab = labels.view(nw_img, N)
         mask = torch.where(lab[:, None, :] != lab[:, :, None], -100.0, 0.0).to(_HP)
-    return attention(qkv, B * nw_img, N, H, dh, scale, bias=bias, mask=mask, row_map=row_map, nw_img=nw_img)
+    return attention(qkv, B * nw_img, N, H, dh, scale, bias=bias, mask=mask, row_map=row_map, nw_img=nw_img,
+                     key_block=None)   # the window kernels take the whole window in one pass
 
 
 def window_attention_tc(qkv, bias_pad, row_map, maskbits, B, nw_img, N, H, dh, scale):
@@ -204,7 +245,7 @@ def window_attention_tc(qkv, bias_pad, row_map, maskbits, B, nw_img, N, H, dh, s
         bits = (maskbits[:, :N, None] >> torch.arange(N, device=maskbits.device)[None, None, :]) & 1
         mask = torch.where(bits.bool(), -100.0, 0.0).to(_HP)
     return attention(qkv, B * nw_img, N, H, dh, scale, bias=bias_pad[:, :N, :N], mask=mask, row_map=row_map,
-                     nw_img=nw_img)
+                     nw_img=nw_img, key_block=None)
 
 
 def patchify(img, p, out_dtype, mean=None, inv_std=None, scale=1.0):

@@ -320,6 +320,59 @@ def _softmax_err(qkv, B, N, H, dh, scale, bias=None, mask=None, row_map=None, nw
     return do, dp, pv, idx if row_map is not None else None
 
 
+def _blocked_softmax_err(s, ds, v, key_block, round_p, u_acc, u_arg=_U):
+    """Bound on |kernel - statement| of O = softmax(s) V for a tensor-core kernel running the online softmax of
+    ``emulate_bf16._softmax_pv`` over ``key_block``-key blocks, with P rounded by ``round_p`` (bf16 or TF32) before
+    P V; before the output's own rounding.  ``s`` (..., Nq, N): the exact scores, ``ds`` the bound on the kernel's
+    error of each, ``v`` (..., N, dh); ``u_acc`` the unit of the P V accumulation, ``u_arg`` that of the roundings of
+    the exponent's argument (its scaling and the subtraction of the running max).  Per query row, with m_b the running
+    max of key j's block, M the row max, c_j = exp(m_b - M) and Z = sum exp(s - M):
+
+    * p_j = exp(s_j - m_b) is off by <= dp_j = p_j (2 max ds + u_arg (|s_j| + |s_j - m_b|) + 2 ulp of exp2) +
+      2^-126 (results below fp32's normal range are flushed): the running maxima only shift the scores, so their
+      error is one more max ds;
+    * tie term: the kernel rounds a value within dp_j of p_j; where round_p(p_j - dp_j) != round_p(p_j + dp_j) that
+      rounding may differ from the statement's by their difference (one spacing of P: ``ulp_bf16``, or TF32's
+      2^(e-11)): (c tie / Z) @ |V|;
+    * the rescale of block b to the row max, c_j, is off by <= eta_j = 2 max ds (the maxima at both ends; between them
+      the alphas' exponents telescope) + u_arg (M - m_b) (their argument roundings) + 6u per rescale (exp2's 2 ulp,
+      the products alpha O and alpha l);
+    * O's numerator: (R eta) @ |V| + gamma_{N + 2 nblocks}(u_acc) R @ |V| with R = c round_p(p) / Z, the statement's P;
+    * the row sum: relative error lam <= sum_j P_j (eta_j + dp_j / p_j) + gamma_{N + 2 nblocks + 3}(u) (its fp32
+      sums and the division O / l), which moves O by (|O| + numerator error) lam."""
+    N = s.shape[-1]
+    nb = -(-N // key_block)
+    blk = F.pad(s, (0, nb * key_block - N), value=-math.inf).unflatten(-1, (nb, key_block)).amax(-1)
+    mb = torch.cummax(blk, dim=-1).values.repeat_interleave(key_block, dim=-1)[..., :N]
+    M = mb[..., -1:]
+    dsm = ds.amax(-1, keepdim=True)
+    p = torch.exp(s - mb)
+    eps = 2 * dsm + u_arg * (s.abs() + (mb - s)) + 4 * _U
+    dp = p * eps + 2.0 ** -126
+    tie = round_p(p + dp) - round_p((p - dp).clamp_min(0.0))
+    c = torch.exp(mb - M)
+    Z = torch.exp(s - M).sum(-1, keepdim=True)
+    eta = 2 * dsm + u_arg * (M - mb) + 6 * _U * nb
+    R = c * round_p(p) / Z
+    av = v.abs()
+    d_num = (R * eta + c * tie / Z) @ av + _gamma(N + 2 * nb, u_acc) * (R @ av)
+    lam = (c * p / Z * (eta + eps)).sum(-1, keepdim=True) + _gamma(N + 2 * nb + 3)
+    return d_num + ((R @ v).abs() + d_num) * lam
+
+
+def _blocked_attention_bound(qkv, B, N, H, dh, scale, round_p):
+    """Per-element bound of the ViT / PiT / TF32 tensor-core attention against ``emulate_bf16.attention`` in 64-key
+    blocks: scores accumulated in the tensor cores (truncating fp32 adds, gamma_{dh+3}: dh products, the scaling by
+    scale log2 e and that constant's rounding), then ``_blocked_softmax_err``.  Computed per chunk of images."""
+    q, k, v = qkv.to(_F64).view(B, N, 3, H, dh).permute(2, 0, 3, 1, 4)
+    out = []
+    for c in emu.image_chunks(B, H, N):
+        s = scale * (q[c] @ k[c].transpose(-1, -2))
+        ds = _gamma(dh + 3, _UT) * scale * (q[c].abs() @ k[c].abs().transpose(-1, -2))
+        out.append(_blocked_softmax_err(s, ds, v[c], emu.KEY_BLOCK, round_p, _UT))
+    return _heads_to_rows(torch.cat(out), B, N, H, dh, None)
+
+
 def _heads_to_rows(o, B, n, H, dh, idx):
     o = o.permute(0, 2, 1, 3).reshape(B * n, H * dh)
     if idx is not None:
@@ -332,14 +385,11 @@ def _heads_to_rows(o, B, n, H, dh, idx):
 def _rule_attention(A):
     qkv, B, N, H, dh = A["qkv"], A["B"], A["N"], A["H"], A["dh"]
     if qkv.dtype == torch.bfloat16:
-        # The tensor-core kernel rounds P to bf16 per 64-key block of its online softmax (relative to the running
-        # max), the reference with the global row max: each side's rounding moves O by <= 2^-9 (P |V|), so the two
-        # differ by <= 2^-8 (P |V|) on top of the fp32 terms.  The flip criterion does not apply: P's roundings
-        # differ by design.  (tests/test_kernels_gpu.py::test_attention_bf16 holds its randn inputs to
-        # 2^-8 max|ref|; on ViT activations that is less than one bf16 ulp of the largest outputs, and an exact
-        # simulation of the per-block rounding exceeds it by up to 1.8x at the same rows as the kernel.)
-        do, _, pv, _ = _softmax_err(qkv, B, N, H, dh, A["scale"], u=_UT)
-        return [("out", _ret, _bounded(_heads_to_rows(do + 2.0 ** -8 * pv, B, N, H, dh, None), flips=False))]
+        # The tensor-core kernel: P rounded to bf16 per 64-key block of its online softmax, as the statement does;
+        # they differ by fp32 arithmetic and, where a P element lies that close to a rounding boundary, by one bf16
+        # spacing of it (_blocked_softmax_err).
+        bound = _blocked_attention_bound(qkv, B, N, H, dh, A["scale"], emu.round_bf16)
+        return [("out", _ret, _bounded(bound))]
     do, dp, _, idx = _softmax_err(qkv, B, N, H, dh, A["scale"], A["bias"], A["mask"], A["row_map"], A["nw_img"])
     outs = [("out", _ret, _bounded(_heads_to_rows(do, B, N, H, dh, idx)))]
     if A["probs"] is not None:

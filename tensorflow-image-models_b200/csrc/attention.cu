@@ -159,13 +159,14 @@ vit_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* 
         }
       }
     }
-    // normalise and write through the (now dead) Q tile in smem for coalesced stores
-    float inv[2];
+    // normalise (O / l correctly rounded) and write through the (now dead) Q tile in smem for coalesced stores
+    float lsum[2], inv[2];
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       float l = l_run[r];
       l += __shfl_xor_sync(0xffffffffu, l, 1);
       l += __shfl_xor_sync(0xffffffffu, l, 2);
+      lsum[r] = l;
       inv[r] = 1.0f / l;
     }
     __syncwarp();
@@ -174,9 +175,9 @@ vit_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* 
     for (int nt = 0; nt < kDH / 8; ++nt) {
       const int r0 = g, r1 = g + 8;
       *reinterpret_cast<uint32_t*>(tile_gen + r0 * 128 + ((nt ^ (r0 & 7)) << 4) + t * 4) =
-          pack_bf16x2(o[nt][0] * inv[0], o[nt][1] * inv[0]);
+          pack_bf16x2(div_rn_by(o[nt][0], lsum[0], inv[0]), div_rn_by(o[nt][1], lsum[0], inv[0]));
       *reinterpret_cast<uint32_t*>(tile_gen + r1 * 128 + ((nt ^ (r1 & 7)) << 4) + t * 4) =
-          pack_bf16x2(o[nt][2] * inv[1], o[nt][3] * inv[1]);
+          pack_bf16x2(div_rn_by(o[nt][2], lsum[1], inv[1]), div_rn_by(o[nt][3], lsum[1], inv[1]));
     }
     __syncwarp();
 #pragma unroll
@@ -352,12 +353,13 @@ vit_attention_tf32_kernel(const float* __restrict__ qkv, float* __restrict__ out
   }
 
   if (!active) return;
-  float inv[2];
+  float lsum[2], inv[2];
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     float l = l_run[r];
     l += __shfl_xor_sync(0xffffffffu, l, 1);
     l += __shfl_xor_sync(0xffffffffu, l, 2);
+    lsum[r] = l;
     inv[r] = 1.0f / l;
   }
   const long ldo = (long)H * kDH;
@@ -368,7 +370,8 @@ vit_attention_tf32_kernel(const float* __restrict__ qkv, float* __restrict__ out
       float* dst = out + ((long)b * N + row) * ldo + h * kDH + 2 * t;
 #pragma unroll
       for (int jd = 0; jd < kDH / 8; ++jd)
-        *reinterpret_cast<float2*>(dst + 8 * jd) = make_float2(o[jd][2 * hr] * inv[hr], o[jd][2 * hr + 1] * inv[hr]);
+        *reinterpret_cast<float2*>(dst + 8 * jd) = make_float2(div_rn_by(o[jd][2 * hr], lsum[hr], inv[hr]),
+                                                               div_rn_by(o[jd][2 * hr + 1], lsum[hr], inv[hr]));
     }
   }
 }

@@ -103,6 +103,14 @@ __device__ __forceinline__ float ex2_approx(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
+// a / l, correctly rounded, given inv = 1.0f / l (itself correctly rounded): q = a inv is within an ulp of a / l, the
+// remainder a - q l is exact in one fma, and q + remainder * inv rounds to the correctly rounded quotient (Markstein).
+// Attention normalises every output of a row by its row sum l: the plain product a * inv would carry the one rounding
+// error of inv into all of them alike, a bias that decides the bf16 rounding of every output near a tie the same way.
+__device__ __forceinline__ float div_rn_by(float a, float l, float inv) {
+  const float q = a * inv;
+  return fmaf(fmaf(-q, l, a), inv, q);
+}
 __device__ __forceinline__ float rcp_approx(float x) {
   float y;
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));

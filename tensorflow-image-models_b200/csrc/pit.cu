@@ -193,20 +193,22 @@ pit_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* 
   cp_async_wait<0>();   // only empty groups can be pending here
   if (!active) return;
 
-  float inv[2];
+  float lsum[2], inv[2];
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     float l = l_run[r];
     l += __shfl_xor_sync(0xffffffffu, l, 1);
     l += __shfl_xor_sync(0xffffffffu, l, 2);
+    lsum[r] = l;
     inv[r] = 1.0f / l;
   }
   uint8_t* tile = smem + q0 * RB;   // this warp's Q rows: read only by this warp, before the key loop
 #pragma unroll
   for (int nt = 0; nt < DH / 8; ++nt) {
-    *reinterpret_cast<uint32_t*>(tile + g * RB + nt * 16 + t * 4) = pack_bf16x2(o[nt][0] * inv[0], o[nt][1] * inv[0]);
+    *reinterpret_cast<uint32_t*>(tile + g * RB + nt * 16 + t * 4) =
+        pack_bf16x2(div_rn_by(o[nt][0], lsum[0], inv[0]), div_rn_by(o[nt][1], lsum[0], inv[0]));
     *reinterpret_cast<uint32_t*>(tile + (g + 8) * RB + nt * 16 + t * 4) =
-        pack_bf16x2(o[nt][2] * inv[1], o[nt][3] * inv[1]);
+        pack_bf16x2(div_rn_by(o[nt][2], lsum[1], inv[1]), div_rn_by(o[nt][3], lsum[1], inv[1]));
   }
   __syncwarp();
   const long ldo = (long)H * DH;

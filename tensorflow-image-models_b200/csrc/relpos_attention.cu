@@ -289,7 +289,8 @@ relpos_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat1
       __nv_bfloat16* dst = dst_img + (long)row * ldo;
 #pragma unroll
       for (int nt = 0; nt < C::NT; ++nt)
-        *reinterpret_cast<uint32_t*>(dst + 8 * nt) = pack_bf16x2(o[nt][2 * hr] * inv, o[nt][2 * hr + 1] * inv);
+        *reinterpret_cast<uint32_t*>(dst + 8 * nt) =
+            pack_bf16x2(div_rn_by(o[nt][2 * hr], l, inv), div_rn_by(o[nt][2 * hr + 1], l, inv));
     }
   }
 }

@@ -3,8 +3,8 @@ oracle/shadow.py.
 
 Each launcher gets
 * a statement at the kernels' storage points, in the emulation's arithmetic (float64 by default):
-  - ``pit_attention_bf16``: the bf16 qkv as stored, softmax(scale q k^T) v with P rounded to bf16 (the emulation's
-    attention), one rounding of the output to bf16;
+  - ``pit_attention_bf16``: the bf16 qkv as stored, softmax(scale q k^T) v with P rounded to bf16 per 64-key block
+    of an online softmax (the emulation's attention), one rounding of the output to bf16;
   - ``pit_pool``: the reference's ConvHeadPooling on the grid rows -- reshape to (B, H, W, C), ZeroPadding2D(1), a
     VALID 3 x 3 / 2 Conv2D with groups = C (torch's grouped convolution: output channel o reads input o // 2), plus
     bias -- one rounding to fp32; and the token rows rounded to bf16 when asked.  The output's token rows belong to
@@ -12,9 +12,9 @@ Each launcher gets
     shows.
 * a derived error bound for the op-by-op shadow harness (``_rule_*``):
   - the attention: the bound of the ViT tensor-core kernel (``shadow._rule_attention``), the same algorithm: fp32
-    scores accumulated in the tensor cores, fp32 online softmax, P rounded to bf16 per 64-key block against the
-    running maximum where the statement rounds against the row maximum (2^-8 P |V| between the two), and the output's
-    own bf16 rounding;
+    scores accumulated in the tensor cores, fp32 online softmax over 64-key blocks with P rounded to bf16 per block
+    against the running maximum, as the statement does (``shadow._blocked_softmax_err``), the output's own bf16
+    rounding and the flip criterion;
   - the pool: nine fp32 fmas onto the bias, gamma_10 (|b| + sum |w| |x|); the bf16 token rows exactly.
 
 ``emulated_pit_ops()`` / ``shadowed_pit_ops()`` are ``emulated_ops()`` / ``shadowed_ops()`` with these launchers

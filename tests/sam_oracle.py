@@ -6,8 +6,9 @@ csrc/relpos_attention.cu) gets
 
 * a float64 statement with the kernels' rounding points (``relpos_attention``): q, k, v are the stored qkv values (bf16
   or fp32), the window padding's keys / values are the stored qkv bias, the relative-position terms use the unscaled q
-  and the fp32 tables as they are; in bf16, P is rounded to bf16 per 64-key block of an online softmax (relative to the
-  running row max) before P V, and the row sum is that of the unrounded P -- what the tensor-core kernel does;
+  and the fp32 tables as they are; in bf16, the online softmax of ``emulate_bf16._softmax_pv`` over 64-key blocks, P
+  rounded to bf16 per block (relative to the running row max) and the row sum of the unrounded P -- what the
+  tensor-core kernel does;
 * a derived error bound for the op-by-op shadow harness (``relpos_bound``).
 
 ``emulated_sam_ops()`` / ``shadowed_sam_ops()`` are ``emulated_ops()`` / ``shadowed_ops()`` with this launcher added.
@@ -20,7 +21,6 @@ from oracle import emulate_bf16 as emu
 from oracle import shadow
 
 _F64 = torch.float64
-_BLOCK = 64
 
 
 def seq_index(gh, gw, window, device=None):
@@ -72,18 +72,7 @@ def relpos_attention(qkv, B, gh, gw, H, dh, scale, rel_h, rel_w, window=0, pad_b
         qh, kh, vh = q[:, :, h], k[:, :, h], v[:, :, h]
         s = scale * (qh @ kh.transpose(-1, -2)) + _rel(qh, rh, rw, ty, tx)
         if qkv.dtype == torch.bfloat16:
-            m = torch.full(s.shape[:-1] + (1,), -torch.inf, dtype=hp, device=s.device)
-            l = torch.zeros_like(m)
-            o = torch.zeros(s.shape[:-1] + (dh,), dtype=hp, device=s.device)
-            for j0 in range(0, s.shape[-1], _BLOCK):
-                sb = s[..., j0:j0 + _BLOCK]
-                m_new = torch.maximum(m, sb.amax(-1, keepdim=True))
-                alpha = torch.exp(m - m_new)
-                p = torch.exp(sb - m_new)
-                l = l * alpha + p.sum(-1, keepdim=True)
-                o = o * alpha + p.to(torch.bfloat16).to(hp) @ vh[..., j0:j0 + _BLOCK, :]
-                m = m_new
-            o = o / l
+            o, _ = emu._softmax_pv(s, vh, emu.round_bf16, emu.KEY_BLOCK)
         else:
             o = torch.softmax(s, dim=-1) @ vh
         outs.append(o)
@@ -97,11 +86,11 @@ def relpos_bound(qkv, B, gh, gw, H, dh, scale, rel_h, rel_w, window=0, pad_bias=
     * each logit s = scale q.k + q.R_h + q.R_w is off by ds <= gamma_{dh+3}(u) scale |q||k| + (gamma_{2dh+3}(u) +
       e_R) (|q||R_h| + |q||R_w|): fp32 accumulation of exact products (u = 2^-23 on the tensor cores, which truncate;
       2^-24 in the SIMT kernel) and, in bf16, R carried as a bf16 hi + lo pair (e_R = 2^-17);
-    * softmax sees differences of logits only, so p_j moves by <= p_j (2 max ds + 4u (|s_j| + |s_j - m|) +
-      gamma_{N+8}): the argument's scaling by log2(e), exp2, the row sum and the division;
-    * O = P V then moves by (dP |V|) + gamma_{N+2} (P |V|);
-    * bf16 only: the kernel rounds P to bf16 per 64-key block relative to the running max, the statement does the same
-      but from exact logits; each side's rounding moves O by <= 2^-9 (P |V|), together <= 2^-8 (P |V|).
+    * bf16 (tensor-core kernel, the statement's online softmax over 64-key blocks): ``shadow._blocked_softmax_err``
+      with 4u per unit of |s_j| + |s_j - m| for the argument (the table sum, its scaling by log2(e), the fma);
+    * fp32 (SIMT kernel, one pass): softmax sees differences of logits only, so p_j moves by <= p_j (2 max ds + 4u
+      (|s_j| + |s_j - m|) + gamma_{N+8}): the argument's scaling by log2(e), exp2, the row sum and the division;
+      O = P V then moves by (dP |V|) + gamma_{N+2} (P |V|).
     This is the bound of the ViT attention (oracle/shadow.py, _rule_attention) with the relative-position terms in the
     logit error."""
     bf16 = qkv.dtype == torch.bfloat16
@@ -115,13 +104,13 @@ def relpos_bound(qkv, B, gh, gw, H, dh, scale, rel_h, rel_w, window=0, pad_bias=
         s = scale * (qh @ kh.transpose(-1, -2)) + _rel(qh, rh, rw, ty, tx)
         ds = (shadow._gamma(dh + 3, u) * scale * (qh.abs() @ kh.abs().transpose(-1, -2))
               + (shadow._gamma(2 * dh + 3, u) + e_r) * _rel(qh.abs(), rh.abs(), rw.abs(), ty, tx))
-        m = s.amax(-1, keepdim=True)
-        p = torch.softmax(s, dim=-1)
-        dp = p * (2 * ds.amax(-1, keepdim=True) + 4 * shadow._U * (s.abs() + (s - m).abs()) + shadow._gamma(N + 8))
-        pv = p @ vh.abs()
-        do = dp @ vh.abs() + shadow._gamma(N + 2) * pv
         if bf16:
-            do = do + 2.0 ** -8 * pv
+            do = shadow._blocked_softmax_err(s, ds, vh, emu.KEY_BLOCK, emu.round_bf16, u, u_arg=4 * shadow._U)
+        else:
+            m = s.amax(-1, keepdim=True)
+            p = torch.softmax(s, dim=-1)
+            dp = p * (2 * ds.amax(-1, keepdim=True) + 4 * shadow._U * (s.abs() + (s - m).abs()) + shadow._gamma(N + 8))
+            do = dp @ vh.abs() + shadow._gamma(N + 2) * (p @ vh.abs())
         outs.append(do)
     return _to_rows(torch.stack(outs, dim=2), idx, B, gh * gw)
 
@@ -129,8 +118,7 @@ def relpos_bound(qkv, B, gh, gw, H, dh, scale, rel_h, rel_w, window=0, pad_bias=
 def _rule_relpos_attention(A):
     bound = relpos_bound(A["qkv"], A["B"], A["gh"], A["gw"], A["H"], A["dh"], A["scale"], A["rel_h"], A["rel_w"],
                          A["window"], A["pad_bias"])
-    # the flip criterion does not apply: the two sides round P from different logits by design
-    return [("out", shadow._ret, shadow._bounded(bound, flips=False))]
+    return [("out", shadow._ret, shadow._bounded(bound))]
 
 
 @contextmanager

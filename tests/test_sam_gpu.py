@@ -71,7 +71,7 @@ def test_relpos_attention_bf16(B, gh, gw, H, dh, window):
     torch.cuda.synchronize()
     ref = relpos_attention(qkv, B, gh, gw, H, dh, scale, rh, rw, window, pad)
     bound = relpos_bound(qkv, B, gh, gw, H, dh, scale, rh, rw, window, pad)
-    ok, worst, _ = shadow.check("relpos_attention", out, ref, shadow._bounded(bound, flips=False))
+    ok, worst, _ = shadow.check("relpos_attention", out, ref, shadow._bounded(bound))
     print(f"relpos bf16 B={B} grid={gh}x{gw} H={H} dh={dh} window={window}: worst {worst:.3f} x bound")
     assert ok, worst
 
@@ -102,7 +102,7 @@ def test_padding_keys_are_keys_not_masked():
     out = sam_ops.relpos_attention(qkv, B, gh, gw, H, dh, scale, rh, rw, window, pad)
     ref = relpos_attention(qkv, B, gh, gw, H, dh, scale, rh, rw, window, pad)
     bound = relpos_bound(qkv, B, gh, gw, H, dh, scale, rh, rw, window, pad)
-    assert shadow.check("relpos_attention", out, ref, shadow._bounded(bound, flips=False))[0]
+    assert shadow.check("relpos_attention", out, ref, shadow._bounded(bound))[0]
     # padding keys masked: the attention of each window over its real tokens only
     x = qkv.double().view(B, gh, gw, 3, H, dh)
     masked = torch.empty(B, gh, gw, H, dh, dtype=torch.float64, device="cuda")
@@ -184,7 +184,7 @@ def test_relpos_attention_bf16_shared_memory_edge(dh, edge):
     out = sam_ops.relpos_attention(qkv, B, edge, edge, H, dh, scale, rh, rw, 0, pad)
     ref = relpos_attention(qkv, B, edge, edge, H, dh, scale, rh, rw, 0, pad)
     bound = relpos_bound(qkv, B, edge, edge, H, dh, scale, rh, rw, 0, pad)
-    assert shadow.check("relpos_attention", out, ref, shadow._bounded(bound, flips=False))[0]
+    assert shadow.check("relpos_attention", out, ref, shadow._bounded(bound))[0]
     qkv, rh, rw, pad = _inputs(B, edge + 1, edge + 1, H, dh, 0, torch.bfloat16)
     with pytest.raises(KernelLibraryError, match="shared memory"):
         sam_ops.relpos_attention(qkv, B, edge + 1, edge + 1, H, dh, scale, rh, rw, 0, pad)

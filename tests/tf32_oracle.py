@@ -9,8 +9,9 @@ fp32.  Inside ``tf32_oracle()``:
   operands (the weights already are), q, k and v, and the softmax numerator P before P V -- and then compute exactly as
   before (float64);
 * the shadow harness's rules for them bound the kernel against that emulation: the fp32 accumulation of exact TF32
-  products (``shadow._UT`` per term, the tensor core truncates), no storage ulp (outputs are fp32), and for attention the
-  per-key-block rounding of P.
+  products (``shadow._UT`` per term, the tensor core truncates), no storage ulp (outputs are fp32), and for attention
+  ``shadow._blocked_softmax_err`` with TF32's spacing of P -- the statement runs the kernel's online softmax over 64-key
+  blocks.
 
 Both take the tf32 branch only while a tf32 model's forward pass runs (``tfimm.backend.lib.tf32_mode``) and the operands
 are fp32; every other call is the unchanged statement and rule.  Enter it outside ``emulated_ops()`` /
@@ -24,13 +25,17 @@ from oracle import emulate_bf16 as emu
 from oracle import shadow
 
 _F64 = torch.float64
-_TF32_U = 2.0 ** -11   # unit roundoff of TF32 (11 significant bits)
 
 
 def round_tf32(t):
     from tfimm.backend.lib import round_tf32 as r
 
     return r(t)
+
+
+def round_p_tf32(p):
+    """P as the TF32 P V product sees it (``cvt.rna`` of the fp32 value), kept in p's dtype."""
+    return round_tf32(p.float()).to(p.dtype)
 
 
 def _tf32_on(*tensors):
@@ -69,11 +74,9 @@ def _emu_attention(base):
         if not _plain_attention(qkv, dh, bias, mask, probs, row_map):
             return base(qkv, B, N, H, dh, scale, bias=bias, mask=mask, probs=probs, row_map=row_map, nw_img=nw_img)
         q, k, v = round_tf32(qkv).to(emu._HP).view(B, N, 3, H, dh).permute(2, 0, 3, 1, 4)
-        s = scale * (q @ k.transpose(-1, -2))
-        p = torch.exp(s - s.amax(dim=-1, keepdim=True))
-        l = p.sum(dim=-1, keepdim=True)                      # the row sum of the unrounded P, as the kernel
-        p = round_tf32(p.float()).to(emu._HP)                # P as the PV product sees it
-        o = (p @ v) / l
+        # the kernel's online softmax: P rounded to TF32 per 64-key block, the row sum of the unrounded P
+        o = torch.cat([emu._softmax_pv(scale * (q[c] @ k[c].transpose(-1, -2)), v[c], round_p_tf32, emu.KEY_BLOCK)[0]
+                       for c in emu.image_chunks(B, H, N)])
         return o.permute(0, 2, 1, 3).reshape(B * N, H * dh).contiguous().to(qkv.dtype)
     return attention
 
@@ -110,13 +113,10 @@ def _rule_attention(base):
         qkv, B, N, H, dh = A["qkv"], A["B"], A["N"], A["H"], A["dh"]
         if not _plain_attention(qkv, dh, A["bias"], A["mask"], A["probs"], A["row_map"]):
             return base(A)
-        # The bf16 branch's argument with TF32's unit roundoff: the kernel rounds P per 64-key block of its online
-        # softmax (relative to the running max), the reference with the global row max; each side's rounding moves P
-        # by <= 2^-11 of itself, so O by <= 2^-11 (P |V|), and the two differ by <= 2^-10 (P |V|) on top of the fp32
-        # terms of the softmax and the accumulations.  q, k, v are rounded identically on both sides.
-        do, _, pv, _ = shadow._softmax_err(round_tf32(qkv), B, N, H, dh, A["scale"], u=shadow._UT)
-        bound = shadow._heads_to_rows(do + 2 * _TF32_U * pv, B, N, H, dh, None)
-        return [("out", shadow._ret, shadow._bounded(bound, flips=False))]
+        # The bf16 branch's bound with P rounded to TF32 (its spacing 2^(e-11)) and q, k, v rounded on both sides; the
+        # output is fp32: its own rounding is the final product's, part of the bound.
+        bound = shadow._blocked_attention_bound(round_tf32(qkv), B, N, H, dh, A["scale"], round_p_tf32)
+        return [("out", shadow._ret, shadow._bounded(bound))]
     return rule
 
 
