@@ -8,13 +8,13 @@
 //
 // bf16 path: one CTA per (image, head, 224-query chunk); K and V of the head are
 // staged once in XOR-swizzled shared memory with cp.async, each warp owns 16-row
-// query tiles and runs a flash-style online softmax over 64-key blocks with
-// mma.sync m16n8k16 (fp32 accumulate, fp32 softmax statistics).
+// query tiles and runs the online softmax of attention_mma.cuh with mma.sync m16n8k16.
 //
 // tf32 path (precision="tf32"): fp32 qkv / out, mma.sync m16n8k8 TF32, K / V streamed in 64-key blocks.
 //
 // fp32 path (precision="fp32" parity mode, and every call with bias / mask / probs / row_map): plain SIMT, one warp
 // per query row.
+#include "attention_mma.cuh"
 #include "common.cuh"
 
 #include <stdlib.h>
@@ -79,8 +79,7 @@ vit_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* 
     float o[kDH / 8][4];
 #pragma unroll
     for (int i = 0; i < kDH / 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
-    float m_run[2] = {-INFINITY, -INFINITY};
-    float l_run[2] = {0.f, 0.f};
+    OnlineSoftmax<false> sm;
 
 #pragma unroll 1
     for (int kb = 0; kb < nblocks; ++kb) {
@@ -114,70 +113,23 @@ vit_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* 
           mx[e >> 1] = fmaxf(mx[e >> 1], val);
         }
       }
-      float alpha[2];
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-        const float m_new = fmaxf(m_run[r], mx[r]);
-        alpha[r] = exp2f(m_run[r] - m_new);
-        m_run[r] = m_new;
-        l_run[r] *= alpha[r];
-      }
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float pv = exp2f(s[nt][e] - m_run[e >> 1]);
-          s[nt][e] = pv;
-          l_run[e >> 1] += pv;
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < kDH / 8; ++i) {
-        o[i][0] *= alpha[0]; o[i][1] *= alpha[0];
-        o[i][2] *= alpha[1]; o[i][3] *= alpha[1];
-      }
-      // O += P V
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
-        if (2 * kk < ntv) {
-          uint32_t a[4];
-          a[0] = pack_bf16x2(s[2 * kk][0], s[2 * kk][1]);
-          a[1] = pack_bf16x2(s[2 * kk][2], s[2 * kk][3]);
-          a[2] = pack_bf16x2(s[2 * kk + 1][0], s[2 * kk + 1][1]);
-          a[3] = pack_bf16x2(s[2 * kk + 1][2], s[2 * kk + 1][3]);
-#pragma unroll
-          for (int jp = 0; jp < kDH / 16; ++jp) {
-            const int row = key0 + kk * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
-            const int chunk = 2 * jp + (lane >> 4);
-            uint32_t v0, v1, v2, v3;
-            ldmatrix_x4_trans(sV + row * 128 + ((chunk ^ (row & 7)) << 4), v0, v1, v2, v3);
-            mma_bf16_16816(o[2 * jp], a, v0, v1);
-            mma_bf16_16816(o[2 * jp + 1], a, v2, v3);
-          }
-        }
-      }
+      sm.update(s, o, mx);
+      pv_bf16(o, s, ntv, lane, [&](int r, int chunk) {
+        const int row = key0 + r;
+        return sV + row * 128 + ((chunk ^ (row & 7)) << 4);
+      });
     }
     // normalise (O / l correctly rounded) and write through the (now dead) Q tile in smem for coalesced stores
-    float lsum[2], inv[2];
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      float l = l_run[r];
-      l += __shfl_xor_sync(0xffffffffu, l, 1);
-      l += __shfl_xor_sync(0xffffffffu, l, 2);
-      lsum[r] = l;
-      inv[r] = 1.0f / l;
-    }
+    const RowNorm n0 = sm.finish(0), n1 = sm.finish(1);
     __syncwarp();
     uint8_t* tile_gen = smem + q0 * 128;
 #pragma unroll
     for (int nt = 0; nt < kDH / 8; ++nt) {
       const int r0 = g, r1 = g + 8;
       *reinterpret_cast<uint32_t*>(tile_gen + r0 * 128 + ((nt ^ (r0 & 7)) << 4) + t * 4) =
-          pack_bf16x2(div_rn_by(o[nt][0], lsum[0], inv[0]), div_rn_by(o[nt][1], lsum[0], inv[0]));
+          pack_bf16x2(n0(o[nt][0]), n0(o[nt][1]));
       *reinterpret_cast<uint32_t*>(tile_gen + r1 * 128 + ((nt ^ (r1 & 7)) << 4) + t * 4) =
-          pack_bf16x2(div_rn_by(o[nt][2], lsum[1], inv[1]), div_rn_by(o[nt][3], lsum[1], inv[1]));
+          pack_bf16x2(n1(o[nt][2]), n1(o[nt][3]));
     }
     __syncwarp();
 #pragma unroll
@@ -207,7 +159,7 @@ int launch_vit_attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, in
   static std::atomic<unsigned long long> attr_devs{0};
   TFIMM_CUDA_OK(set_max_dynamic_smem(kernel, 227 * 1024, attr_devs));
   dim3 grid((N + ROWS - 1) / ROWS, H, B);
-  kernel<<<grid, NW * 32, smem, stream>>>(qkv, out, N, H, scale * 1.4426950408889634f);
+  kernel<<<grid, NW * 32, smem, stream>>>(qkv, out, N, H, scale * kLog2e);
   TFIMM_LAUNCH_OK("vit_attention_bf16_kernel");
   return kOk;
 }
@@ -215,8 +167,8 @@ int launch_vit_attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, in
 // ---- TF32 path (precision="tf32"): fp32 qkv / out, TF32 tensor-core products ----
 // One CTA per (image, head, 128-query chunk), 8 warps of 16 query rows.  fp32 K / V of a whole head do not fit shared
 // memory at N = 577 (295 KB), so they stream through a double-buffered cp.async ring of 64-key blocks shared by the
-// warps; each warp runs the flash-style online softmax of the bf16 kernel (fp32 statistics, exp2) with mma.sync
-// m16n8k8 TF32.  Q, K, V are rounded to TF32 (cvt.rna) as their fragments are loaded; P is rounded before PV.
+// warps; each warp runs the online softmax of attention_mma.cuh with mma.sync m16n8k8 TF32.  Q, K, V are rounded to
+// TF32 (cvt.rna) as their fragments are loaded; P is rounded before PV.
 //
 // Fragment bookkeeping: the contraction index of an m16n8k8 product is free to permute as long as A and B agree.
 //   S = Q K^T: k-step ks covers dims 8 ks .. 8 ks + 7; logical k = t <-> dim 8 ks + 2t, k = t + 4 <-> dim 8 ks + 2t + 1,
@@ -273,8 +225,7 @@ vit_attention_tf32_kernel(const float* __restrict__ qkv, float* __restrict__ out
   float o[kDH / 8][4];
 #pragma unroll
   for (int i = 0; i < kDH / 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
-  float m_run[2] = {-INFINITY, -INFINITY};
-  float l_run[2] = {0.f, 0.f};
+  OnlineSoftmax<false> sm;
 
 #pragma unroll 1
   for (int kb = 0; kb < nblocks; ++kb) {
@@ -315,30 +266,7 @@ vit_attention_tf32_kernel(const float* __restrict__ qkv, float* __restrict__ out
           mx[e >> 1] = fmaxf(mx[e >> 1], val);
         }
       }
-      float alpha[2];
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-        const float m_new = fmaxf(m_run[r], mx[r]);
-        alpha[r] = exp2f(m_run[r] - m_new);
-        m_run[r] = m_new;
-        l_run[r] *= alpha[r];
-      }
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float pv = exp2f(s[nt][e] - m_run[e >> 1]);
-          s[nt][e] = pv;
-          l_run[e >> 1] += pv;   // the row sum of the unrounded fp32 P
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < kDH / 8; ++i) {
-        o[i][0] *= alpha[0]; o[i][1] *= alpha[0];
-        o[i][2] *= alpha[1]; o[i][3] *= alpha[1];
-      }
+      sm.update(s, o, mx);
       // O += P V
 #pragma unroll
       for (int nt = 0; nt < 8; ++nt) {
@@ -353,15 +281,7 @@ vit_attention_tf32_kernel(const float* __restrict__ qkv, float* __restrict__ out
   }
 
   if (!active) return;
-  float lsum[2], inv[2];
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    float l = l_run[r];
-    l += __shfl_xor_sync(0xffffffffu, l, 1);
-    l += __shfl_xor_sync(0xffffffffu, l, 2);
-    lsum[r] = l;
-    inv[r] = 1.0f / l;
-  }
+  const RowNorm nrm[2] = {sm.finish(0), sm.finish(1)};
   const long ldo = (long)H * kDH;
 #pragma unroll
   for (int hr = 0; hr < 2; ++hr) {
@@ -370,8 +290,7 @@ vit_attention_tf32_kernel(const float* __restrict__ qkv, float* __restrict__ out
       float* dst = out + ((long)b * N + row) * ldo + h * kDH + 2 * t;
 #pragma unroll
       for (int jd = 0; jd < kDH / 8; ++jd)
-        *reinterpret_cast<float2*>(dst + 8 * jd) = make_float2(div_rn_by(o[jd][2 * hr], lsum[hr], inv[hr]),
-                                                               div_rn_by(o[jd][2 * hr + 1], lsum[hr], inv[hr]));
+        *reinterpret_cast<float2*>(dst + 8 * jd) = make_float2(nrm[hr](o[jd][2 * hr]), nrm[hr](o[jd][2 * hr + 1]));
     }
   }
 }
@@ -471,7 +390,7 @@ int tfimm_b200_attention_tf32(const float* qkv, float* out, int B, int N, int H,
   TFIMM_CUDA_OK(set_max_dynamic_smem(vit_attention_tf32_kernel, (int)kTfSmemBytes, attr_devs));
   dim3 grid((N + kTfRows - 1) / kTfRows, H, B);
   vit_attention_tf32_kernel<<<grid, kTfWarps * 32, kTfSmemBytes, stream>>>(qkv, out, N, H,
-                                                                           scale * 1.4426950408889634f);
+                                                                           scale * kLog2e);
   TFIMM_LAUNCH_OK("vit_attention_tf32_kernel");
   return kOk;
 }

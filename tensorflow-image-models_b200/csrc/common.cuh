@@ -96,6 +96,8 @@ int make_tmap_2d(CUtensorMap* map, const void* ptr, int dtype, uint64_t rows, ui
 // ----------------------------------------------------------------------------
 // Small device math
 // ----------------------------------------------------------------------------
+constexpr float kLog2e = 1.4426950408889634f;
+
 #if defined(__CUDACC__)
 
 __device__ __forceinline__ float ex2_approx(float x) {

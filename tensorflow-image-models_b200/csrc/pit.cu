@@ -9,12 +9,9 @@
 //     scores, so they add nothing to the row sums and zero V rows to the output.
 //   - Shared-memory rows are DH + 8 bf16 long: DH / 8 + 1 sixteen-byte chunks, an odd number, so the eight row
 //     addresses of every ldmatrix phase fall on eight different 16-byte bank groups at DH 32, 48 and 64.
-//   - S = Q K^T with mma.sync m16n8k16 (bf16 in, fp32 accumulate): one ldmatrix.x4 feeds two 8-key tiles for one k16
-//     step.  The online softmax is flash-style in fp32: the row maximum is taken on the raw scores, and each score
-//     costs one fma (scale log2 e folded in) and one ex2.approx.  P is rounded to bf16 per 64-key block, relative to
-//     the running maximum, as the ViT kernels do; the row sum l is of the unrounded P.
-//   - O += P V: P stays in registers (the S accumulator layout is the A fragment layout); V comes by ldmatrix.trans,
-//     two 8-column tiles per x4.  DH 48 is three k16 steps for S and six n8 tiles for O.
+//   - S = Q K^T, the online softmax and O += P V are attention_mma.cuh's, on mma.sync m16n8k16.  The row maximum is
+//     taken on the raw scores, and each score costs one fma (scale log2 e folded in) and one ex2.approx.ftz.  DH 48 is
+//     three k16 steps for S and six n8 tiles for O.
 //   - The normalised tile is staged through the warp's own (dead) Q rows in shared memory and stored as 16-byte
 //     chunks; rows past T are not stored.
 // pit_pool_kernel  the 3 x 3 / 2, groups = C, 2C-filter convolution with zero padding 1, plus bias, fp32 on the CUDA
@@ -23,6 +20,7 @@
 //   consecutive output pixels.  Consecutive threads take consecutive c4 of one pixel, so loads and stores are
 //   coalesced.  The grid rows are read from and written to the token streams in place: no reshape, pad or concat.
 //   When asked, the same launch copies the token rows of x to bf16 (the operand of the token Dense in bf16 models).
+#include "attention_mma.cuh"
 #include "common.cuh"
 #include "tfimm_b200_pit.h"
 
@@ -100,8 +98,7 @@ pit_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* 
   float o[DH / 8][4];
 #pragma unroll
   for (int i = 0; i < DH / 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
-  float m_run[2] = {-INFINITY, -INFINITY};   // in units of scale log2 e
-  float l_run[2] = {0.f, 0.f};
+  OnlineSoftmax<true> sm;
 
 #pragma unroll 1
   for (int kb = 0; kb < nblocks; ++kb) {
@@ -113,26 +110,11 @@ pit_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* 
     const uint32_t sV = sK + kKeys * RB;
     const int key0 = kb * kKeys;
     const int nvalid = min(kKeys, T - key0);
+    const int ntiles = (nvalid + 7) >> 3;   // 8-key tiles holding a key < T
 
     float s[8][4];
-#pragma unroll
-    for (int nt = 0; nt < 8; ++nt) s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
-#pragma unroll
-    for (int np = 0; np < 4; ++np) {
-      if (np * 16 < nvalid) {
-#pragma unroll
-        for (int ks = 0; ks < DH / 16; ++ks) {
-          const int row = np * 16 + (lane >> 4) * 8 + (lane & 7);
-          const int chunk = ks * 2 + ((lane >> 3) & 1);
-          uint32_t k0, k1, k2, k3;
-          ldmatrix_x4(sK + row * RB + chunk * 16, k0, k1, k2, k3);
-          mma_bf16_16816(s[2 * np], qf[ks], k0, k1);
-          mma_bf16_16816(s[2 * np + 1], qf[ks], k2, k3);
-        }
-      }
-    }
+    qk_bf16(s, qf, ntiles, lane, [&](int row, int chunk) { return sK + row * RB + chunk * 16; });
     if (nvalid < kKeys) {
-      // accumulator element e of tile nt: row g + 8 (e / 2), key 8 nt + 2 t + e % 2
 #pragma unroll
       for (int nt = 0; nt < 8; ++nt)
 #pragma unroll
@@ -145,70 +127,20 @@ pit_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* 
       mx[0] = fmaxf(mx[0], fmaxf(s[nt][0], s[nt][1]));
       mx[1] = fmaxf(mx[1], fmaxf(s[nt][2], s[nt][3]));
     }
-    float alpha[2], neg_m[2];
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-      const float m_new = fmaxf(m_run[r], mx[r] * scale_log2);   // every block has a key < T: finite
-      alpha[r] = ex2_approx(m_run[r] - m_new);
-      m_run[r] = m_new;
-      neg_m[r] = -m_new;
-      l_run[r] *= alpha[r];
-    }
-#pragma unroll
-    for (int nt = 0; nt < 8; ++nt) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float p = ex2_approx(fmaf(s[nt][e], scale_log2, neg_m[e >> 1]));
-        s[nt][e] = p;
-        l_run[e >> 1] += p;
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < DH / 8; ++i) {
-      o[i][0] *= alpha[0]; o[i][1] *= alpha[0];
-      o[i][2] *= alpha[1]; o[i][3] *= alpha[1];
-    }
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      if (kk * 16 < nvalid) {
-        uint32_t a[4];
-        a[0] = pack_bf16x2(s[2 * kk][0], s[2 * kk][1]);
-        a[1] = pack_bf16x2(s[2 * kk][2], s[2 * kk][3]);
-        a[2] = pack_bf16x2(s[2 * kk + 1][0], s[2 * kk + 1][1]);
-        a[3] = pack_bf16x2(s[2 * kk + 1][2], s[2 * kk + 1][3]);
-#pragma unroll
-        for (int jp = 0; jp < DH / 16; ++jp) {
-          const int row = kk * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
-          const int chunk = 2 * jp + (lane >> 4);
-          uint32_t v0, v1, v2, v3;
-          ldmatrix_x4_trans(sV + row * RB + chunk * 16, v0, v1, v2, v3);
-          mma_bf16_16816(o[2 * jp], a, v0, v1);
-          mma_bf16_16816(o[2 * jp + 1], a, v2, v3);
-        }
-      }
-    }
+    sm.update(s, o, mx, scale_log2);
+    pv_bf16(o, s, ntiles, lane, [&](int row, int chunk) { return sV + row * RB + chunk * 16; });
   }
   cp_async_wait<0>();   // only empty groups can be pending here
   if (!active) return;
 
-  float lsum[2], inv[2];
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    float l = l_run[r];
-    l += __shfl_xor_sync(0xffffffffu, l, 1);
-    l += __shfl_xor_sync(0xffffffffu, l, 2);
-    lsum[r] = l;
-    inv[r] = 1.0f / l;
-  }
+  const RowNorm n0 = sm.finish(0), n1 = sm.finish(1);
   uint8_t* tile = smem + q0 * RB;   // this warp's Q rows: read only by this warp, before the key loop
 #pragma unroll
   for (int nt = 0; nt < DH / 8; ++nt) {
     *reinterpret_cast<uint32_t*>(tile + g * RB + nt * 16 + t * 4) =
-        pack_bf16x2(div_rn_by(o[nt][0], lsum[0], inv[0]), div_rn_by(o[nt][1], lsum[0], inv[0]));
+        pack_bf16x2(n0(o[nt][0]), n0(o[nt][1]));
     *reinterpret_cast<uint32_t*>(tile + (g + 8) * RB + nt * 16 + t * 4) =
-        pack_bf16x2(div_rn_by(o[nt][2], lsum[1], inv[1]), div_rn_by(o[nt][3], lsum[1], inv[1]));
+        pack_bf16x2(n1(o[nt][2]), n1(o[nt][3]));
   }
   __syncwarp();
   const long ldo = (long)H * DH;
@@ -228,7 +160,7 @@ int launch_pit_attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, in
   static std::atomic<unsigned long long> attr_devs{0};
   TFIMM_CUDA_OK(set_max_dynamic_smem(kernel, AttnShape<DH>::kSmem, attr_devs));
   const dim3 grid((T + kRows - 1) / kRows, H, B);
-  kernel<<<grid, kWarps * 32, AttnShape<DH>::kSmem, stream>>>(qkv, out, T, H, scale * 1.4426950408889634f);
+  kernel<<<grid, kWarps * 32, AttnShape<DH>::kSmem, stream>>>(qkv, out, T, H, scale * kLog2e);
   TFIMM_LAUNCH_OK("pit_attention_bf16_kernel");
   return kOk;
 }

@@ -17,9 +17,10 @@
 // double-buffered cp.async ring of 64-key blocks (a head's K / V at N = 4096 are 1 MB).  Each warp first computes
 // q . R for all 2S - 1 offsets of both tables with the tensor cores (R split into bf16 hi + lo parts, so the products
 // carry R to ~2^-17) and scatters them into a per-row [S_h | S_w] table in shared memory; the main loop adds the two
-// gathered terms to the logits.  mma.sync m16n8k16 for every product, fp32 online softmax, P rounded to bf16 per block.
+// gathered terms to the logits.  mma.sync m16n8k16 for every product; the online softmax is attention_mma.cuh's.
 //
 // fp32 path (precision="fp32", and head dims the bf16 kernel does not take): SIMT, one warp per query row.
+#include "attention_mma.cuh"
 #include "common.cuh"
 
 namespace tfimm {
@@ -28,7 +29,6 @@ namespace {
 constexpr int kRpWarps = 8;
 constexpr int kRpRows = kRpWarps * 16;
 constexpr int kRpKeys = 64;
-constexpr float kLog2e = 1.4426950408889634f;
 
 template <int DH>
 struct RpCfg {
@@ -175,8 +175,7 @@ relpos_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat1
   float o[C::NT][4];
 #pragma unroll
   for (int i = 0; i < C::NT; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
-  float m_run[2] = {-INFINITY, -INFINITY};
-  float l_run[2] = {0.f, 0.f};
+  OnlineSoftmax<false> sm;
   const float* rel0 = relbuf + g * rs;
   const float* rel1 = relbuf + (g + 8) * rs;
 
@@ -194,21 +193,7 @@ relpos_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat1
       const uint32_t sV = sK + kRpKeys * C::LDS * 2;
       const int key0 = kb * kRpKeys;
       float s[8][4];
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt) s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
-      // S = q k^T: one ldmatrix.x4 gives the k16 B fragments of two key tiles
-#pragma unroll
-      for (int np = 0; np < 4; ++np) {
-#pragma unroll
-        for (int ks = 0; ks < C::KS; ++ks) {
-          const int row = 16 * np + (lane & 7) + ((lane >> 4) << 3);
-          const int chunk = 2 * ks + ((lane >> 3) & 1);
-          uint32_t k0, k1, k2, k3;
-          ldmatrix_x4(sK + (row * C::LDS + chunk * 8) * 2, k0, k1, k2, k3);
-          mma_bf16_16816(s[2 * np], qf[ks], k0, k1);
-          mma_bf16_16816(s[2 * np + 1], qf[ks], k2, k3);
-        }
-      }
+      qk_bf16(s, qf, 8, lane, [&](int row, int chunk) { return sK + (row * C::LDS + chunk * 8) * 2; });
       // logits in log2 units: scale q.k + rel_h + rel_w; keys >= N masked; row max
       float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
@@ -228,48 +213,8 @@ relpos_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat1
           mx[1] = fmaxf(mx[1], s[nt][2 + c]);
         }
       }
-      float alpha[2];
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-        const float m_new = fmaxf(m_run[r], mx[r]);
-        alpha[r] = exp2f(m_run[r] - m_new);
-        m_run[r] = m_new;
-        l_run[r] *= alpha[r];
-      }
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float pv = exp2f(s[nt][e] - m_run[e >> 1]);
-          s[nt][e] = pv;
-          l_run[e >> 1] += pv;
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < C::NT; ++i) {
-        o[i][0] *= alpha[0]; o[i][1] *= alpha[0];
-        o[i][2] *= alpha[1]; o[i][3] *= alpha[1];
-      }
-      // O += P V (P rounded to bf16)
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
-        uint32_t a[4];
-        a[0] = pack_bf16x2(s[2 * kk][0], s[2 * kk][1]);
-        a[1] = pack_bf16x2(s[2 * kk][2], s[2 * kk][3]);
-        a[2] = pack_bf16x2(s[2 * kk + 1][0], s[2 * kk + 1][1]);
-        a[3] = pack_bf16x2(s[2 * kk + 1][2], s[2 * kk + 1][3]);
-        const int row = kk * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
-#pragma unroll
-        for (int jp = 0; jp < C::NT / 2; ++jp) {
-          const int chunk = 2 * jp + (lane >> 4);
-          uint32_t v0, v1, v2, v3;
-          ldmatrix_x4_trans(sV + (row * C::LDS + chunk * 8) * 2, v0, v1, v2, v3);
-          mma_bf16_16816(o[2 * jp], a, v0, v1);
-          mma_bf16_16816(o[2 * jp + 1], a, v2, v3);
-        }
-      }
+      sm.update(s, o, mx);
+      pv_bf16(o, s, 8, lane, [&](int row, int chunk) { return sV + (row * C::LDS + chunk * 8) * 2; });
     }
     __syncthreads();   // every warp is done with this stage before block kb + 2 is loaded into it
   }
@@ -279,10 +224,7 @@ relpos_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat1
   __nv_bfloat16* dst_img = out + (long)b * geo.gh * geo.gw * ldo + h * DH + 2 * t;
 #pragma unroll
   for (int hr = 0; hr < 2; ++hr) {
-    float l = l_run[hr];
-    l += __shfl_xor_sync(0xffffffffu, l, 1);
-    l += __shfl_xor_sync(0xffffffffu, l, 2);
-    const float inv = 1.0f / l;
+    const RowNorm nrm = sm.finish(hr);
     const int j = q0 + g + 8 * hr;
     const int row = j < N ? geo.row(seq, j) : -1;
     if (row >= 0) {
@@ -290,7 +232,7 @@ relpos_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat1
 #pragma unroll
       for (int nt = 0; nt < C::NT; ++nt)
         *reinterpret_cast<uint32_t*>(dst + 8 * nt) =
-            pack_bf16x2(div_rn_by(o[nt][2 * hr], l, inv), div_rn_by(o[nt][2 * hr + 1], l, inv));
+            pack_bf16x2(nrm(o[nt][2 * hr]), nrm(o[nt][2 * hr + 1]));
     }
   }
 }

@@ -13,6 +13,7 @@
 // shared memory with cp.async; S = q k^T on mma.sync m16n8k16 (ROWS / 16 query tiles x ROWS / 8 key tiles), then
 // + relative-position bias[h] (+ -100 between tokens of different shift regions), fp32 softmax in
 // registers, P (bf16) V on mma.sync, 4-byte stores of the 16 x 32 output tile.
+#include "attention_mma.cuh"
 #include "common.cuh"
 
 namespace tfimm {
@@ -76,7 +77,6 @@ window_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat1
 
   const int mtiles = (N + 15) >> 4;
   const int ntiles = (N + 7) >> 3;   // key tiles with at least one valid key (<= NT)
-  const float l2e = 1.4426950408889634f;
 
 #pragma unroll 1
   for (int mt = 0; mt < mtiles; ++mt) {
@@ -121,16 +121,13 @@ window_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat1
         } else if (key < N) {
           val = 0.f;  // padded query rows: keep finite, result is discarded
         }
-        s[nt][e] = val * l2e;
+        s[nt][e] = val * kLog2e;
         mx[e >> 1] = fmaxf(mx[e >> 1], s[nt][e]);
       }
     }
     float sum[2] = {0.f, 0.f};
 #pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-    }
+    for (int r = 0; r < 2; ++r) mx[r] = quad_max(mx[r]);
 #pragma unroll
     for (int nt = 0; nt < NT; ++nt) {
 #pragma unroll
@@ -142,34 +139,11 @@ window_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat1
     }
     float inv[2];
 #pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      float l = sum[r];
-      l += __shfl_xor_sync(0xffffffffu, l, 1);
-      l += __shfl_xor_sync(0xffffffffu, l, 2);
-      inv[r] = 1.0f / l;
-    }
+    for (int r = 0; r < 2; ++r) inv[r] = RowNorm(sum[r]).inv;
     float o[4][4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
-#pragma unroll
-    for (int kk = 0; kk < NT / 2; ++kk) {
-      if (2 * kk < ntiles) {
-        uint32_t a[4];
-        a[0] = pack_bf16x2(s[2 * kk][0], s[2 * kk][1]);
-        a[1] = pack_bf16x2(s[2 * kk][2], s[2 * kk][3]);
-        a[2] = pack_bf16x2(s[2 * kk + 1][0], s[2 * kk + 1][1]);
-        a[3] = pack_bf16x2(s[2 * kk + 1][2], s[2 * kk + 1][3]);
-#pragma unroll
-        for (int jp = 0; jp < 2; ++jp) {
-          const int row = kk * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
-          const int chunk = 2 * jp + (lane >> 4);
-          uint32_t v0, v1, v2, v3;
-          ldmatrix_x4_trans(sV + wswz(row, chunk), v0, v1, v2, v3);
-          mma_bf16_16816(o[2 * jp], a, v0, v1);
-          mma_bf16_16816(o[2 * jp + 1], a, v2, v3);
-        }
-      }
-    }
+    pv_bf16(o, s, ntiles, lane, [&](int row, int chunk) { return sV + wswz(row, chunk); });
     __nv_bfloat16* obase = out + img * L * ((long)H * kWDH) + (long)h * kWDH;
 #pragma unroll
     for (int nt = 0; nt < 4; ++nt) {
