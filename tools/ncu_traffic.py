@@ -30,6 +30,8 @@ FAMILIES = [
     ("gn1_partials", "gn1_partials"), ("poolformer_mixer", "poolformer_mixer"), ("gn1_apply", "gn1_apply"),
     ("gemm_f32", "gemm_f32"),
     ("pit_attention_bf16", "pit_attention_bf16"), ("pit_pool", "pit_pool"),
+    # before "dwconv_*": the ConvMixer kernel's name contains "dwconv"
+    ("convmixer_dwconv", "convmixer_dwconv"),
     # before "attention_f32": the Segment Anything kernels' names contain it
     ("relpos_attention_bf16", "relpos_attention_bf16"), ("relpos_attention_f32", "relpos_attention_f32"),
     ("vit_attention_tf32", "attention_tf32"), ("vit_attention", "attention_bf16"), ("attention_cls", "attention_cls_bf16"), ("attention_f32", "attention_f32"),
