@@ -193,28 +193,31 @@ def attention(qkv, B, N, H, dh, scale, bias=None, mask=None, probs=None, row_map
     """bf16 qkv: P rounded to bf16 per block of ``key_block`` keys (the tensor-core kernels; the window kernels pass
     None: one block); fp32 qkv: the SIMT kernel's unrounded softmax over the whole row."""
     dt = qkv.dtype
-    x = qkv.to(_HP)
+    x = qkv
     if row_map is not None:  # Swin: rows of window w of image b live at row_map[w*N + i] of that image's tokens
         nimg = B // nw_img
         tok = nw_img * N
         idx = (torch.arange(nimg, device=x.device)[:, None] * tok + row_map.long()[None, :]).reshape(-1)
         x = x[idx]
-    q, k, v = x.view(B, N, 3, H, dh).permute(2, 0, 3, 1, 4)
+    x = x.view(B, N, 3, H, dh)
     round_p = round_bf16 if dt == torch.bfloat16 else None
-    if bias is None and mask is None and probs is None:
-        o = torch.cat([_softmax_pv(scale * (q[c] @ k[c].transpose(-1, -2)), v[c], round_p,
-                                   key_block if round_p is not None else None)[0]
-                       for c in image_chunks(B, H, N)])
-    else:
+    kb = key_block if round_p is not None else None
+
+    def chunk(c):
+        """(scores, v) of the images (windows) of slice c, in float64"""
+        q, k, v = x[c].to(_HP).permute(2, 0, 3, 1, 4)
         s = scale * (q @ k.transpose(-1, -2))
         if bias is not None:
             s = s + bias.to(_HP)[None]
-        if mask is not None:
-            nm = mask.shape[0]
-            s = (s.view(B // nm, nm, H, N, N) + mask.to(_HP)[None, :, None]).view(B, H, N, N)
-        o, p = _softmax_pv(s, v, round_p, key_block if round_p is not None else None)
-        if probs is not None:
-            probs.copy_(p)
+        if mask is not None:   # image (window) b takes mask[b % nm]
+            s = s + mask.to(_HP)[torch.arange(c.start, c.stop, device=s.device) % mask.shape[0]][:, None]
+        return s, v
+
+    if probs is None:
+        o = torch.cat([_softmax_pv(*chunk(c), round_p, kb)[0] for c in image_chunks(B, H, N)])
+    else:
+        o, p = _softmax_pv(*chunk(slice(0, B)), round_p, kb)
+        probs.copy_(p)
     o = o.permute(0, 2, 1, 3).reshape(B * N, H * dh)
     if row_map is not None:
         out = torch.empty_like(o)

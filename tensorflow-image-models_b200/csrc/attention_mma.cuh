@@ -9,7 +9,7 @@
 //     l = alpha l + sum_j p_j,     O = alpha O + round(p) V.
 // P is rounded (to bf16, or to TF32) per block, against the running maximum, and l sums the unrounded fp32 p.  At the
 // end out = O / l, correctly rounded (div_rn_by).  Window attention is a single block of up to 144 keys with no running
-// state, normalised by o * (1 / l).
+// state, normalised the same way.
 //
 // Everything here works on one warp's 16-row accumulator tile of m16n8k16 / m16n8k8: thread (g, t) = (lane / 4,
 // lane % 4) holds rows g and g + 8, and element e of 8-column tile nt is row g + 8 (e / 2), column 8 nt + 2 t + e % 2.

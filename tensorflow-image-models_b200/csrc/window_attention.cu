@@ -12,7 +12,7 @@
 // One warp per (window, head): q/k/v (N x 32 bf16 each, zero-padded to ROWS = 64 / 144 rows) staged in swizzled
 // shared memory with cp.async; S = q k^T on mma.sync m16n8k16 (ROWS / 16 query tiles x ROWS / 8 key tiles), then
 // + relative-position bias[h] (+ -100 between tokens of different shift regions), fp32 softmax in
-// registers, P (bf16) V on mma.sync, 4-byte stores of the 16 x 32 output tile.
+// registers, P (bf16) V on mma.sync, O / l correctly rounded (RowNorm), 4-byte stores of the 16 x 32 output tile.
 #include "attention_mma.cuh"
 #include "common.cuh"
 
@@ -137,9 +137,7 @@ window_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat1
         sum[e >> 1] += pv;
       }
     }
-    float inv[2];
-#pragma unroll
-    for (int r = 0; r < 2; ++r) inv[r] = RowNorm(sum[r]).inv;
+    const RowNorm nrm[2] = {RowNorm(sum[0]), RowNorm(sum[1])};
     float o[4][4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
@@ -149,10 +147,10 @@ window_attention_bf16_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat1
     for (int nt = 0; nt < 4; ++nt) {
       if (r0 < N)
         *reinterpret_cast<uint32_t*>(obase + (long)s_rows[warp][r0] * ((long)H * kWDH) + nt * 8 + 2 * t) =
-            pack_bf16x2(o[nt][0] * inv[0], o[nt][1] * inv[0]);
+            pack_bf16x2(nrm[0](o[nt][0]), nrm[0](o[nt][1]));
       if (r1 < N)
         *reinterpret_cast<uint32_t*>(obase + (long)s_rows[warp][r1] * ((long)H * kWDH) + nt * 8 + 2 * t) =
-            pack_bf16x2(o[nt][2] * inv[1], o[nt][3] * inv[1]);
+            pack_bf16x2(nrm[1](o[nt][2]), nrm[1](o[nt][3]));
     }
   }
 }

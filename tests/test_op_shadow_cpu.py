@@ -82,9 +82,8 @@ def test_float32_standin_passes_every_shadowed_launch(rehearsal, name, precision
     for census in rehearsal[(name, precision)]:
         assert census.rows
         census.assert_ok()
-        # the cited bounds are exceptions: everything else is held to the derived per-element rule
-        assert all(r["cite"] is None for r in census.rows if r["op"] not in (
-            "window_attention", "window_attention_tc", "mlp_fused"))
+        # the fused MLP's cited bound is the one exception: everything else is held to the derived per-element rule
+        assert all(r["cite"] is None for r in census.rows if r["op"] != "mlp_fused")
 
 
 def test_census_reaches_every_launcher(rehearsal):
