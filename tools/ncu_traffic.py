@@ -32,7 +32,9 @@ FAMILIES = [
     ("pit_attention_bf16", "pit_attention_bf16"), ("pit_pool", "pit_pool"),
     # before "dwconv_*": the ConvMixer kernel's name contains "dwconv"
     ("convmixer_dwconv", "convmixer_dwconv"),
-    # before "attention_f32": the Segment Anything kernels' names contain it
+    ("pvt_sr_attention_bf16", "pvt_sr_attention_bf16"), ("pvt_embed_norm", "pvt_embed_norm"),
+    # before "attention_f32": the PVT and Segment Anything kernels' names contain it
+    ("pvt_sr_attention_f32", "pvt_sr_attention_f32"),
     ("relpos_attention_bf16", "relpos_attention_bf16"), ("relpos_attention_f32", "relpos_attention_f32"),
     ("vit_attention_tf32", "attention_tf32"), ("vit_attention", "attention_bf16"), ("attention_cls", "attention_cls_bf16"), ("attention_f32", "attention_f32"),
     ("window_attention", "window_attention_bf16"),
