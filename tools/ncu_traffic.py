@@ -32,6 +32,9 @@ FAMILIES = [
     ("pit_attention_bf16", "pit_attention_bf16"), ("pit_pool", "pit_pool"),
     # before "dwconv_*": the ConvMixer kernel's name contains "dwconv"
     ("convmixer_dwconv", "convmixer_dwconv"),
+    # PVT v2's head-dim-32 instances (template argument 32) before the PVT head-dim-64 ones
+    ("pvt_sr_attention_bf16_kernelILi32E", "pvt_v2_sr_attention_bf16"),
+    ("pvt_sr_attention_f32_kernelILi32E", "pvt_v2_sr_attention_f32"), ("pvt_v2_conv_mlp", "pvt_v2_conv_mlp_bf16"),
     ("pvt_sr_attention_bf16", "pvt_sr_attention_bf16"), ("pvt_embed_norm", "pvt_embed_norm"),
     # before "attention_f32": the PVT and Segment Anything kernels' names contain it
     ("pvt_sr_attention_f32", "pvt_sr_attention_f32"),
