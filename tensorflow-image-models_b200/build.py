@@ -51,7 +51,8 @@ def build(force: bool = False, verbose: bool = False, defines=(), out: Path = No
                                             ROOT.parent / "include" / "tfimm_b200_pit.h",
                                             ROOT.parent / "include" / "tfimm_b200_convmixer.h",
                                             ROOT.parent / "include" / "tfimm_b200_pvt.h",
-                                            ROOT.parent / "include" / "tfimm_b200_pvt_v2.h"]
+                                            ROOT.parent / "include" / "tfimm_b200_pvt_v2.h",
+                                            ROOT.parent / "include" / "tfimm_b200_cait.h"]
     stamp = OBJ_DIR / "stamp.txt"
     digest = _digest(sources + headers)
     if not force and LIB.exists() and stamp.exists() and stamp.read_text() == digest:

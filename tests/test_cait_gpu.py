@@ -1,0 +1,324 @@
+"""CaiT on the H100: the talking-heads kernels (bf16 mma.sync at every H of the family, fp32 SIMT) and class attention
+against their float64 statements within the derived bounds (sequence lengths 1 and 2, the 32- and 16-key block edges
++- 1, every family length up to 2304, logits near +-80, a row whose maximum is in the last key block, mixing weights
+of both signs up to 2), guard regions around every output, bitwise determinism, and the ten registrations in every
+precision, launch by launch under the shadow harness."""
+import dataclasses
+import sys
+from contextlib import nullcontext
+from pathlib import Path
+
+import pytest
+import torch
+
+pytestmark = pytest.mark.gpu
+
+HERE = Path(__file__).resolve().parent
+if str(HERE) not in sys.path:
+    sys.path.insert(0, str(HERE))
+
+import cait_oracle as co  # noqa: E402
+from tf32_oracle import tf32_oracle  # noqa: E402
+
+NAMES = ["cait_xxs24_224", "cait_xxs24_384", "cait_xxs36_224", "cait_xxs36_384", "cait_xs24_384", "cait_s24_224",
+         "cait_s24_384", "cait_s36_384", "cait_m36_384", "cait_m48_448"]
+# N: one and two keys, the bf16 kernel's 32-key block edges +- 1 (the fp32 kernel's 16-key ones fall inside), the
+# family's 196, 576 and 784, and 2304 (cait_m48_448's table interpolated to 768 px)
+LENGTHS = [1, 2, 15, 17, 31, 32, 33, 63, 65, 196, 576, 784, 2304]
+HEADS = [4, 6, 8, 16]
+
+
+@pytest.fixture
+def cait():
+    with co.cait_registered() as mod:
+        yield mod
+
+
+def _inputs(B, N, H, dh, seed, std=1.0, wmax=2.0):
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    qkv = (torch.randn((B * N, 3 * H * dh), generator=g, device="cuda") * std).to(torch.bfloat16)
+    mix = [(torch.rand((H, H), generator=g, device="cuda") * 2 - 1) * wmax * (dh ** -0.5 if i == 0 else 1.0)
+           for i in range(2)]
+    bias = [torch.randn((H,), generator=g, device="cuda") for _ in range(2)]
+    return qkv, mix[0], bias[0], mix[1], bias[1]
+
+
+def _batch(N):
+    return 1 if N >= 576 else 2
+
+
+@pytest.mark.parametrize("N", LENGTHS)
+@pytest.mark.parametrize("H", HEADS)
+def test_talking_heads_bf16_against_float64(H, N):
+    """Every output within the derived bound (cait_oracle.talking_heads_bound) and the flip criterion."""
+    from tfimm.backend import cait_ops
+
+    B = _batch(N)
+    qkv, wl, bl, ww, bw = _inputs(B, N, H, 48, seed=97 * H + N)
+    with co.shadowed_cait_ops() as census:
+        cait_ops.talking_heads_bf16(qkv, wl, bl, ww, bw, B, N, H, 48)
+    census.assert_ok()
+    assert census.ops() == {"talking_heads_bf16"}
+
+
+@pytest.mark.parametrize("N", LENGTHS)
+@pytest.mark.parametrize("H", HEADS)
+def test_talking_heads_f32_against_float64(H, N):
+    from tfimm.backend import cait_ops
+
+    B = _batch(N)
+    qkv, wl, bl, ww, bw = _inputs(B, N, H, 48, seed=89 * H + N)
+    with co.shadowed_cait_ops() as census:
+        cait_ops.talking_heads_f32(qkv.float(), wl, bl, ww, bw, B, N, H, 48)
+    census.assert_ok()
+    assert census.ops() == {"talking_heads_f32"}
+
+
+@pytest.mark.parametrize("H,dh", [(1, 4), (2, 64), (3, 32), (12, 64), (16, 64)])
+def test_talking_heads_f32_other_shapes(H, dh):
+    from tfimm.backend import cait_ops
+
+    for N in (1, 17, 200):
+        qkv, wl, bl, ww, bw = _inputs(2, N, H, dh, seed=H * dh + N)
+        with co.shadowed_cait_ops() as census:
+            cait_ops.talking_heads_f32(qkv.float(), wl, bl, ww, bw, 2, N, H, dh)
+        census.assert_ok()
+
+
+@pytest.mark.parametrize("N", [65, 197, 784])
+@pytest.mark.parametrize("H", HEADS)
+def test_talking_heads_large_logits_and_late_maximum(H, N):
+    """Mixed logits near +-80, so the running maxima move by tens and the rescales matter; every query's maximum on the
+    last key (in the partial last block) for every g: a key along all queries (and the next-to-last key against them),
+    with a positive, diagonally dominant mix."""
+    from tfimm.backend import cait_ops
+
+    B, dh = 2, 48
+    qkv, _, bl, ww, bw = _inputs(B, N, H, dh, seed=7 * H + N)
+    x = qkv.float().view(B, N, 3, H, dh)
+    x[:, :, 0] = x[:, :, 0].abs() * 3.0
+    x[:, :, 1] *= 3.0
+    x[:, N - 1, 1] = 3.0      # the largest logit of every row, in the last key block
+    x[:, N - 2, 1] = -3.0     # the smallest
+    qkv = x.reshape(B * N, -1).to(torch.bfloat16)
+    g = torch.Generator(device="cuda").manual_seed(N)
+    wl = torch.eye(H, device="cuda") * 0.6 + torch.rand((H, H), generator=g, device="cuda") * 0.2
+    q, k = qkv.double().view(B, N, 3, H, dh)[:, :, 0], qkv.double().view(B, N, 3, H, dh)[:, :, 1]
+    S = torch.einsum("bihd,bjhd->bhij", q, k)
+    wl = (wl.double() * 80.0 / torch.einsum("bhij,hg->bgij", S, wl.double()).abs().max()).float()
+    L = torch.einsum("bhij,hg->bgij", S, wl.double())
+    assert 79 < L.max().item() <= 80.01 and L.min().item() < -60
+    assert (L.argmax(-1) == N - 1).all()
+    with co.shadowed_cait_ops() as census:
+        cait_ops.talking_heads_bf16(qkv, wl, bl, ww, bw, B, N, H, dh)
+        cait_ops.talking_heads_f32(qkv.float(), wl, bl, ww, bw, B, N, H, dh)
+    census.assert_ok()
+
+
+@pytest.mark.parametrize("T", [1, 2, 197, 577, 785, 2305])
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32])
+def test_class_attention_against_float64(T, dtype):
+    from tfimm.backend import cait_ops
+
+    g = torch.Generator(device="cuda").manual_seed(T)
+    for H, dh in ((16, 48), (4, 48), (6, 32), (2, 64)):
+        B = 3
+        q = (torch.randn((B, H * dh), generator=g, device="cuda") * 2).to(dtype)
+        kv = (torch.randn((B * T, 2 * H * dh), generator=g, device="cuda") * 2).to(dtype)
+        with co.shadowed_cait_ops() as census:
+            cait_ops.class_attention(q, kv, B, T, H, dh, dh ** -0.5)
+        census.assert_ok()
+
+
+def test_guard_regions_untouched():
+    """Outputs written into the middle of larger buffers: the guard cells on both sides keep their pattern."""
+    from tfimm.backend import cait_ops, lib
+
+    h = cait_ops.load()
+    G = 4096
+    pattern = -1232.0   # exact in bf16
+
+    def buffer(n, dtype):
+        buf = torch.full((n + 2 * G,), pattern, device="cuda").to(dtype)
+        return buf, buf[G:G + n]
+
+    for H in HEADS:
+        B, N = 2, 197
+        qkv, wl, bl, ww, bw = _inputs(B, N, H, 48, seed=H)
+        args = [t.data_ptr() for t in (wl, bl, ww, bw)]
+        buf, out = buffer(B * N * H * 48, torch.bfloat16)
+        assert h.tfimm_b200_cait_talking_heads_bf16(qkv.data_ptr(), out.data_ptr(), *args, B, N, H, 48, None) == 0
+        fbuf, fout = buffer(B * N * H * 48, torch.float32)
+        q32 = qkv.float()
+        assert h.tfimm_b200_cait_talking_heads_f32(q32.data_ptr(), fout.data_ptr(), *args, B, N, H, 48, None) == 0
+        torch.cuda.synchronize()
+        for g in (buf, fbuf):
+            assert (g[:G] == pattern).all() and (g[-G:] == pattern).all()
+        assert torch.equal(out.view(B * N, -1), cait_ops.talking_heads_bf16(qkv, wl, bl, ww, bw, B, N, H, 48))
+        assert torch.equal(fout.view(B * N, -1), cait_ops.talking_heads_f32(q32, wl, bl, ww, bw, B, N, H, 48))
+    for dtype, code in ((torch.bfloat16, lib.BF16), (torch.float32, lib.F32)):
+        B, T, H, dh = 3, 197, 4, 48
+        q = torch.randn((B, H * dh), device="cuda").to(dtype)
+        kv = torch.randn((B * T, 2 * H * dh), device="cuda").to(dtype)
+        buf, out = buffer(B * H * dh, dtype)
+        assert h.tfimm_b200_cait_class_attention(q.data_ptr(), kv.data_ptr(), out.data_ptr(), code, B, T, H, dh,
+                                                 dh ** -0.5, None) == 0
+        torch.cuda.synchronize()
+        assert (buf[:G] == pattern).all() and (buf[-G:] == pattern).all()
+        assert torch.equal(out.view(B, -1), cait_ops.class_attention(q, kv, B, T, H, dh, dh ** -0.5))
+    B, N, D = 3, 196, 192
+    xbuf, x = buffer(B * N * D, torch.float32)
+    x.copy_(torch.randn(B * N * D, device="cuda"))
+    pos = torch.randn((N, D), device="cuda")
+    ref = x.view(B, N, D) + pos
+    cait_ops.add_pos(x.view(B * N, D), pos, B, N)
+    torch.cuda.synchronize()
+    assert (xbuf[:G] == pattern).all() and (xbuf[-G:] == pattern).all() and torch.equal(x.view(B, N, D), ref)
+
+
+def test_determinism():
+    from tfimm.backend import cait_ops
+
+    for H, N in ((4, 576), (6, 577), (8, 196), (16, 784)):
+        qkv, wl, bl, ww, bw = _inputs(4, N, H, 48, seed=N)
+        a = cait_ops.talking_heads_bf16(qkv, wl, bl, ww, bw, 4, N, H, 48)
+        b = cait_ops.talking_heads_bf16(qkv, wl, bl, ww, bw, 4, N, H, 48)
+        assert torch.equal(a.view(torch.int16), b.view(torch.int16))
+        a = cait_ops.talking_heads_f32(qkv.float(), wl, bl, ww, bw, 4, N, H, 48)
+        b = cait_ops.talking_heads_f32(qkv.float(), wl, bl, ww, bw, 4, N, H, 48)
+        assert torch.equal(a.view(torch.int32), b.view(torch.int32))
+
+
+def test_images_are_independent():
+    """A batch of 8 equals its images run one at a time, bit for bit (no state leaks between CTAs of other images)."""
+    from tfimm.backend import cait_ops
+
+    for H, N in ((4, 196), (16, 577)):
+        qkv, wl, bl, ww, bw = _inputs(8, N, H, 48, seed=H + N)
+        full = cait_ops.talking_heads_bf16(qkv, wl, bl, ww, bw, 8, N, H, 48)
+        for b in (0, 5, 7):
+            one = cait_ops.talking_heads_bf16(qkv[b * N:(b + 1) * N].contiguous(), wl, bl, ww, bw, 1, N, H, 48)
+            assert torch.equal(full[b * N:(b + 1) * N], one)
+
+
+# ------------------------------------------------------------------------------------------------------ models
+def _model(name, precision, seed=11, **kw):
+    import tfimm
+    from oracle import params
+
+    cfg = dataclasses.replace(tfimm.models.registry.model_config(name), **kw)
+    m = tfimm.create_model(name, precision=precision, device="cuda") if not kw else \
+        type(tfimm.create_model(name, device="meta"))(cfg, precision=precision, device="cuda")
+    w = co.randomise(params.random_params({k: tuple(v.shape) for k, v in m.params.items()}, seed=seed), seed + 1)
+    m.load_weights_dict(w)
+    return m, w
+
+
+def _nerr(a, b):
+    return ((a.double() - b.double()).abs().max() / b.double().abs().max()).item()
+
+
+@pytest.mark.parametrize("precision", ["bf16", "tf32", "fp32"])
+@pytest.mark.parametrize("name", NAMES)
+def test_shadowed_forward_registered(cait, name, precision):
+    """Each registration in each precision at batch 1, every launch inside its bound; the trace shows which attention
+    kernel ran."""
+    from oracle import params
+    from tfimm.backend import ops
+
+    m, _ = _model(name, precision)
+    x = params.test_images(1, *m.cfg.input_size).cuda()
+    ops.trace = []
+    try:
+        with (tf32_oracle() if precision == "tf32" else nullcontext()), co.shadowed_cait_ops() as census:
+            m(x)
+        names = {t[0] for t in ops.trace}
+    finally:
+        ops.trace = None
+    census.assert_ok()
+    assert {"cait_class_attention", "cait_add_pos"} <= names
+    want = "cait_talking_heads_bf16" if precision == "bf16" else "cait_talking_heads_f32"
+    other = "cait_talking_heads_f32" if precision == "bf16" else "cait_talking_heads_bf16"
+    assert want in names and other not in names, names
+
+
+@pytest.mark.parametrize("name", ["cait_xxs24_224", "cait_s24_224", "cait_m36_384"])
+def test_fp32_logits_match_oracle(cait, name):
+    from oracle import cait as oc
+    from oracle import params
+
+    m, w = _model(name, "fp32")
+    x = params.test_images(2, *m.cfg.input_size)
+    y = m(x.cuda()).cpu()
+    ref = oc.forward(m.cfg, w, x)
+    err = _nerr(y, ref)
+    print(f"FP32 {name}: normalised max error {err:.2e}")
+    assert err < 2e-5, err
+
+
+def _rms(a, b):
+    return ((a.double() - b.double()).pow(2).mean().sqrt() / b.double().pow(2).mean().sqrt()).item()
+
+
+@pytest.mark.parametrize("name", ["cait_xxs24_224", "cait_s24_224"])
+def test_bf16_error_budget(cait, name):
+    """The kernels diverge from the ideal bf16 graph (emulated, float64 arithmetic, the engine's bf16 storage points) by
+    no more than 1.6 x the float64-vs-float32 emulation floor (B1), and the engine is no farther from the float64
+    oracle than the ideal bf16 graph is (B2)."""
+    from oracle import cait as oc
+    from oracle import params
+
+    m, w = _model(name, "bf16")
+    x = params.test_images(2, *m.cfg.input_size)
+    xc = x.cuda()
+    y = m(xc).double().cpu()
+    with co.emulated_cait_ops():
+        y_ideal = m(xc).double().cpu()
+    with co.emulated_cait_ops(arithmetic=torch.float32):
+        y_ideal32 = m(xc).double().cpu()
+    ref = oc.forward(m.cfg, w, x)
+    r_eng, r_ideal, r_kern, r_floor = _rms(y, ref), _rms(y_ideal, ref), _rms(y, y_ideal), _rms(y_ideal32, y_ideal)
+    print(f"BUDGET {name}: rms engine-vs-oracle {r_eng:.2e} | ideal-vs-oracle {r_ideal:.2e} | engine-vs-ideal "
+          f"{r_kern:.2e} | floor {r_floor:.2e}")
+    assert r_kern < 1.6 * r_floor + 1e-4, (r_kern, r_floor)      # B1
+    assert r_eng < 1.25 * r_ideal + 1e-4, (r_eng, r_ideal)       # B2
+
+
+@pytest.mark.parametrize("name", ["cait_xxs24_224", "cait_xs24_384"])
+def test_cuda_graph_uint8_and_features(cait, name):
+    from tfimm.backend import ops
+
+    m, _ = _model(name, "bf16")
+    cfg = m.cfg
+    x = torch.rand((4, *cfg.input_size, 3), device="cuda")
+    eager = m(x)
+    run = m.cuda_graph(4)
+    assert torch.equal(run(x), eager)
+    u8 = torch.randint(0, 256, (2, *cfg.input_size, 3), dtype=torch.uint8, device="cuda")
+    mean = torch.tensor(cfg.mean, device="cuda")
+    std = torch.tensor(cfg.std, device="cuda")
+    ref = m((u8.float() / 255.0 - mean) / std)
+    err = _nerr(m(u8), ref)
+    print(f"UINT8 {name}: normalised max error vs float input {err:.2e}")
+    assert err < 2e-2, err   # the first bf16 rounding of the two pixel paths differs
+    y, feats = m(x[:2], return_features=True)
+    assert list(feats) == m.feature_names
+    assert torch.equal(feats["logits"], y)
+    assert feats["features_all"].shape == (2, cfg.nb_patches + 1, cfg.embed_dim)
+    assert feats[f"block_{cfg.nb_blocks - 1}"].shape == (2, cfg.nb_patches, cfg.embed_dim)
+    assert ops.launch_count > 0
+
+
+def test_interpolate_input_and_headless(cait):
+    """A non-square input through interpolate_input (13 x 17 patches on an H = 6 model) and nb_classes = 0, in fp32
+    against the oracle."""
+    from oracle import cait as oc
+    from oracle import params
+
+    for name, kw, size in (("cait_xs24_384", dict(interpolate_input=True), (208, 272)),
+                           ("cait_xxs24_224", dict(nb_classes=0), (224, 224))):
+        m, w = _model(name, "fp32", seed=4, **kw)
+        x = params.test_images(2, *size)
+        y = m(x.cuda()).cpu()
+        ref = oc.forward(m.cfg, w, x)
+        assert y.shape == ref.shape and _nerr(y, ref) < 2e-5, (name, _nerr(y, ref))

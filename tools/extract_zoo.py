@@ -21,7 +21,7 @@ from pathlib import Path
 REFERENCE = Path("/root/reference")
 OUT = Path(__file__).resolve().parent.parent / "tensorflow-image-models_b200" / "tfimm" / "architectures" / "zoo"
 FAMILIES = ["vit", "swin", "convnext", "efficientnet", "resnet", "mlp_mixer", "poolformer", "pit", "convmixer", "pvt",
-            "pvt_v2"]
+            "pvt_v2", "cait"]
 
 
 class _Meta(type):

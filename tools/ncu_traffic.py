@@ -30,6 +30,8 @@ FAMILIES = [
     ("gn1_partials", "gn1_partials"), ("poolformer_mixer", "poolformer_mixer"), ("gn1_apply", "gn1_apply"),
     ("gemm_f32", "gemm_f32"),
     ("pit_attention_bf16", "pit_attention_bf16"), ("pit_pool", "pit_pool"),
+    ("cait_talking_heads_bf16", "cait_talking_heads_bf16"), ("cait_talking_heads_f32", "cait_talking_heads_f32"),
+    ("cait_class_attn", "cait_class_attention"), ("cait_add_pos", "cait_add_pos"),
     # before "dwconv_*": the ConvMixer kernel's name contains "dwconv"
     ("convmixer_dwconv", "convmixer_dwconv"),
     # PVT v2's head-dim-32 instances (template argument 32) before the PVT head-dim-64 ones
