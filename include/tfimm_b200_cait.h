@@ -1,7 +1,7 @@
 /* tfimm_b200 -- C ABI of the CaiT family's kernels (csrc/cait.cu), in libtfimm_b200.so beside the core entry points of
  * tfimm_b200.h, with the same conventions: device pointers owned by the caller, a status return (0 = OK, else a
- * TFIMM_ERR_* code with tfimm_b200_last_error()), the stream last.  The in-tree binding is
- * tensorflow-image-models_b200/tfimm/backend/cait_ops.py.
+ * TFIMM_ERR_* code with tfimm_b200_last_error()), the stream last.  The in-tree ctypes table is in
+ * tensorflow-image-models_b200/tfimm/backend/lib.py, the launchers in cait_ops.py.
  *
  * Talking-heads attention (tfimm/architectures/cait.py:207-258), per image and query:
  *     L_g  = sum_h wl[h, g] (q_h . k_h) + bl[g]                 (log2 units: the caller folds dh^-0.5 log2 e into wl

@@ -1,7 +1,8 @@
 /* tfimm_b200 -- C ABI of the ConvMixer family's kernel (csrc/convmixer.cu), in libtfimm_b200.so beside the core entry
  * points of tfimm_b200.h, with the same conventions: device pointers owned by the caller, channels-last tensors, a
  * status return (0 = OK, else a TFIMM_ERR_* code with tfimm_b200_last_error()), the stream last.
- * The in-tree binding is tensorflow-image-models_b200/tfimm/backend/convmixer_ops.py. */
+ * The in-tree ctypes table is in tensorflow-image-models_b200/tfimm/backend/lib.py, the launchers in
+ * convmixer_ops.py. */
 #ifndef TFIMM_B200_CONVMIXER_H_
 #define TFIMM_B200_CONVMIXER_H_
 

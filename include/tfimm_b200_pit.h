@@ -1,7 +1,7 @@
 /* tfimm_b200 -- C ABI of the PiT family's kernels (csrc/pit.cu), in libtfimm_b200.so beside the core entry points of
  * tfimm_b200.h, with the same conventions: device pointers owned by the caller, a status return (0 = OK, else a
- * TFIMM_ERR_* code with tfimm_b200_last_error()), the stream last.  The in-tree binding is
- * tensorflow-image-models_b200/tfimm/backend/pit_ops.py.
+ * TFIMM_ERR_* code with tfimm_b200_last_error()), the stream last.  The in-tree ctypes table is in
+ * tensorflow-image-models_b200/tfimm/backend/lib.py, the launchers in pit_ops.py.
  *
  * The residual stream of image b is rows b * T .. b * T + T - 1 of an fp32 (B * T, C) matrix: nb_tokens special tokens
  * (class, then distillation) followed by the H x W grid in row-major order (tfimm/architectures/pit.py:345-349). */

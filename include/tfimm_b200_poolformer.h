@@ -1,7 +1,8 @@
 /* tfimm_b200 -- C ABI of the PoolFormer family's kernels (csrc/poolformer.cu), in libtfimm_b200.so beside the core
  * entry points of tfimm_b200.h, with the same conventions: device pointers owned by the caller, channels-last fp32
  * residual stream, a status return (0 = OK, else a TFIMM_ERR_* code with tfimm_b200_last_error()), the stream last.
- * The in-tree binding is tensorflow-image-models_b200/tfimm/backend/poolformer_ops.py.
+ * The in-tree ctypes table is in tensorflow-image-models_b200/tfimm/backend/lib.py, the launchers in
+ * poolformer_ops.py.
  *
  * GroupNorm with one group (tfimm/layers/norm.py:22-101, norm_layer "group_norm_1grp", eps 1e-5, biased variance)
  * normalises over a whole image.  Its statistics are kept as PARTIALS: image b's H * W * C values, flattened, are split

@@ -1,7 +1,7 @@
 /* tfimm_b200 -- C ABI of the PVT family's kernels (csrc/pvt.cu), in libtfimm_b200.so beside the core entry points of
  * tfimm_b200.h, with the same conventions: device pointers owned by the caller, a status return (0 = OK, else a
- * TFIMM_ERR_* code with tfimm_b200_last_error()), the stream last.  The in-tree binding is
- * tensorflow-image-models_b200/tfimm/backend/pvt_ops.py.
+ * TFIMM_ERR_* code with tfimm_b200_last_error()), the stream last.  The in-tree ctypes table is in
+ * tensorflow-image-models_b200/tfimm/backend/lib.py, the launchers in pvt_ops.py.
  *
  * Spatial-reduction attention (the reference's SpatialReductionAttention): the queries come from all N tokens of an
  * image, the keys and values from N' tokens (the stage grid reduced by a stride-sr convolution, or the tokens

@@ -1,7 +1,7 @@
 /* tfimm_b200 -- C ABI of the PVT v2 family's kernels (csrc/pvt_v2.cu), in libtfimm_b200.so beside the core entry points
  * of tfimm_b200.h, with the same conventions: device pointers owned by the caller, a status return (0 = OK, else a
- * TFIMM_ERR_* code with tfimm_b200_last_error()), the stream last.  The in-tree binding is
- * tensorflow-image-models_b200/tfimm/backend/pvt_v2_ops.py. */
+ * TFIMM_ERR_* code with tfimm_b200_last_error()), the stream last.  The in-tree ctypes table is in
+ * tensorflow-image-models_b200/tfimm/backend/lib.py, the launchers in pvt_v2_ops.py. */
 #ifndef TFIMM_B200_PVT_V2_H_
 #define TFIMM_B200_PVT_V2_H_
 

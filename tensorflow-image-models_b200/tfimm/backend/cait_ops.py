@@ -3,27 +3,14 @@ attention dispatch.
 
 Same conventions as ``tfimm.backend.ops``: torch CUDA tensors in, one library call on the operands' device's current
 stream, counted in ``ops.launch_count`` and bracketed by CUDA events when ``ops.trace`` is set.  Nothing falls back to
-torch ops.  The entry points live in ``libtfimm_b200.so`` but not in ``lib.SIGNATURES``: their ctypes table is here
-and is bound on ``lib.load()``'s handle at first use.
+torch ops.  ``lib.load()`` types their entry points with all the others.
 """
-import ctypes
 import math
 
 import torch
 
 from . import lib as _lib
 from . import ops as _ops
-
-_P, _I, _F = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
-
-SIGNATURES = {
-    "tfimm_b200_cait_talking_heads_bf16": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
-    "tfimm_b200_cait_talking_heads_f32": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
-    "tfimm_b200_cait_class_attention": [_P, _P, _P, _I, _I, _I, _I, _I, _F, _P],
-    "tfimm_b200_cait_add_pos": [_P, _P, _I, _I, _I, _P],
-}
-# trace family of each entry point (bench.py's roofline rows, tools/ncu_traffic.py)
-TRACE_FAMILY = {name: name[len("tfimm_b200_"):] for name in SIGNATURES}
 
 # (H, dh) of the bf16 talking-heads kernel's instantiations: every registered CaiT
 BF16_HEADS = (4, 6, 8, 16)
@@ -34,26 +21,6 @@ F32_HEADS = (1, 2, 3, 4, 6, 8, 12, 16)
 CLS_HEAD_DIMS = (32, 48, 64)
 
 LOG2E = math.log2(math.e)
-
-_bound = None
-
-
-def load():
-    """The library handle with this module's entry points typed (once per handle)."""
-    global _bound
-    handle = _lib.load()
-    if _bound is not handle:
-        for name, argtypes in SIGNATURES.items():
-            fn = getattr(handle, name)
-            fn.argtypes = argtypes
-            fn.restype = _I
-        _bound = handle
-    return handle
-
-
-def _call(name, dev, *args, flops=0.0, nbytes=0.0):
-    load()
-    _ops._call(name, dev, *args, flops=flops, nbytes=nbytes, family=TRACE_FAMILY[name])
 
 
 def f32_supported(H, dh):
@@ -94,9 +61,9 @@ def talking_heads_bf16(qkv, wl, bl, ww, bw, B, N, H, dh):
         (qkv.dtype, qkv.shape, (B, N, H, dh))
     _check_mix(wl, bl, ww, bw, H)
     out = torch.empty((B * N, H * dh), device=qkv.device, dtype=torch.bfloat16)
-    _call("tfimm_b200_cait_talking_heads_bf16", dev, qkv.data_ptr(), out.data_ptr(), wl.data_ptr(), bl.data_ptr(),
-          ww.data_ptr(), bw.data_ptr(), B, N, H, dh, flops=talking_heads_flops(B, N, H, dh),
-          nbytes=talking_heads_nbytes(qkv, out, H))
+    _ops._call("tfimm_b200_cait_talking_heads_bf16", dev, qkv.data_ptr(), out.data_ptr(), wl.data_ptr(), bl.data_ptr(),
+               ww.data_ptr(), bw.data_ptr(), B, N, H, dh, flops=talking_heads_flops(B, N, H, dh),
+               nbytes=talking_heads_nbytes(qkv, out, H))
     return out
 
 
@@ -107,9 +74,9 @@ def talking_heads_f32(qkv, wl, bl, ww, bw, B, N, H, dh):
         (qkv.dtype, qkv.shape, (B, N, H, dh))
     _check_mix(wl, bl, ww, bw, H)
     out = torch.empty((B * N, H * dh), device=qkv.device, dtype=torch.float32)
-    _call("tfimm_b200_cait_talking_heads_f32", dev, qkv.data_ptr(), out.data_ptr(), wl.data_ptr(), bl.data_ptr(),
-          ww.data_ptr(), bw.data_ptr(), B, N, H, dh, flops=talking_heads_flops(B, N, H, dh),
-          nbytes=talking_heads_nbytes(qkv, out, H))
+    _ops._call("tfimm_b200_cait_talking_heads_f32", dev, qkv.data_ptr(), out.data_ptr(), wl.data_ptr(), bl.data_ptr(),
+               ww.data_ptr(), bw.data_ptr(), B, N, H, dh, flops=talking_heads_flops(B, N, H, dh),
+               nbytes=talking_heads_nbytes(qkv, out, H))
     return out
 
 
@@ -121,8 +88,8 @@ def class_attention(q, kv, B, T, H, dh, scale):
     assert q.dtype == kv.dtype and q.shape == (B, D) and q.stride(1) == 1 and q.stride(0) == D, (q.shape, q.stride())
     assert kv.is_contiguous() and kv.shape == (B * T, 2 * D), (kv.shape, (B, T, D))
     out = torch.empty((B, D), device=q.device, dtype=q.dtype)
-    _call("tfimm_b200_cait_class_attention", dev, q.data_ptr(), kv.data_ptr(), out.data_ptr(), _ops._code(q), B, T,
-          H, dh, float(scale), flops=4.0 * B * T * D, nbytes=_ops._nbytes(q, kv, out))
+    _ops._call("tfimm_b200_cait_class_attention", dev, q.data_ptr(), kv.data_ptr(), out.data_ptr(), _ops._code(q), B, T,
+               H, dh, float(scale), flops=4.0 * B * T * D, nbytes=_ops._nbytes(q, kv, out))
     return out
 
 
@@ -132,8 +99,8 @@ def add_pos(x, pos, B, N):
     D = x.shape[1]
     assert x.dtype == pos.dtype == torch.float32 and x.is_contiguous() and pos.is_contiguous(), (x.dtype, pos.dtype)
     assert x.shape == (B * N, D) and pos.shape == (N, D), (x.shape, pos.shape, (B, N))
-    _call("tfimm_b200_cait_add_pos", dev, x.data_ptr(), pos.data_ptr(), B, N, D, flops=float(B * N * D),
-          nbytes=4.0 * (2 * B * N * D + N * D))
+    _ops._call("tfimm_b200_cait_add_pos", dev, x.data_ptr(), pos.data_ptr(), B, N, D, flops=float(B * N * D),
+               nbytes=4.0 * (2 * B * N * D + N * D))
     return x
 
 

@@ -2,42 +2,15 @@
 
 Same conventions as ``tfimm.backend.ops``: torch CUDA tensors in, one library call on the operands' device's current
 stream, counted in ``ops.launch_count`` and bracketed by CUDA events when ``ops.trace`` is set.  Nothing falls back to
-torch ops.  The entry point lives in ``libtfimm_b200.so`` but not in ``lib.SIGNATURES``: its ctypes table is here and is
-bound on ``lib.load()``'s handle at first use.
+torch ops.  ``lib.load()`` types its entry point with all the others.
 """
-import ctypes
-
 import torch
 
-from . import lib as _lib
 from . import ops as _ops
-
-_P, _I = ctypes.c_void_p, ctypes.c_int
-
-SIGNATURES = {
-    "tfimm_b200_convmixer_dwconv": [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P],
-}
-# trace family of each entry point (bench.py's roofline rows, tools/ncu_traffic.py)
-TRACE_FAMILY = {name: name[len("tfimm_b200_"):] for name in SIGNATURES}
 
 # what the kernel takes (csrc/convmixer.cu): the entry point refuses anything else with TFIMM_ERR_UNSUPPORTED
 KERNEL_SIZES = (7, 9)
 CHANNEL_MULTIPLE = 32
-
-_bound = None
-
-
-def load():
-    """The library handle with this module's entry points typed (once per handle)."""
-    global _bound
-    handle = _lib.load()
-    if _bound is not handle:
-        for name, argtypes in SIGNATURES.items():
-            fn = getattr(handle, name)
-            fn.argtypes = argtypes
-            fn.restype = _I
-        _bound = handle
-    return handle
 
 
 def supported(C, k) -> bool:
@@ -66,9 +39,7 @@ def dwconv(a, s_in, t_in, taps, bias, s1, t1, act, out_dtype):
         raise ValueError(f"convmixer_dwconv takes kernel sizes {KERNEL_SIZES} and C % {CHANNEL_MULTIPLE} == 0 "
                          f"(got k={k}, C={C})")
     y = torch.empty((B, H, W, C), device=a.device, dtype=out_dtype)
-    load()
     _ops._call("tfimm_b200_convmixer_dwconv", dev, a.data_ptr(), s_in.data_ptr(), t_in.data_ptr(), taps.data_ptr(),
                bias.data_ptr(), s1.data_ptr(), t1.data_ptr(), y.data_ptr(), _ops._code(y), B, H, W, C, k,
-               _ops.act_code(act), flops=2.0 * B * H * W * C * k * k, nbytes=dwconv_nbytes(B, H, W, C, k, out_dtype),
-               family=TRACE_FAMILY["tfimm_b200_convmixer_dwconv"])
+               _ops.act_code(act), flops=2.0 * B * H * W * C * k * k, nbytes=dwconv_nbytes(B, H, W, C, k, out_dtype))
     return y

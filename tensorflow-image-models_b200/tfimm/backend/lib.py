@@ -1,4 +1,5 @@
-"""ctypes binding of ``libtfimm_b200.so`` (C ABI declared in ``include/tfimm_b200.h``).
+"""ctypes binding of ``libtfimm_b200.so`` (C ABI declared in ``include/tfimm_b200.h`` and the family headers
+``include/tfimm_b200_<family>.h``).
 
 The shared object is built in-tree by ``tensorflow-image-models_b200/build.py``.  Loading it
 does not need a GPU (cudart is linked statically and the driver entry points are resolved
@@ -28,6 +29,7 @@ _F = _c.c_float
 
 # name -> argtypes; restype is int (status) unless listed in _SPECIAL
 SIGNATURES = {
+    # include/tfimm_b200.h
     "tfimm_b200_gemm_bf16": [_P, _I, _P, _I, _P, _P, _P, _I, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P],
     "tfimm_b200_conv_bf16": [_P, _P, _I, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P],
     "tfimm_b200_gemm_f32": [_P, _I, _P, _I, _P, _P, _P, _I, _P, _I, _I, _I, _I, _I, _I, _P],
@@ -69,6 +71,28 @@ SIGNATURES = {
     "tfimm_b200_gemm_glu_bf16": [_P, _I, _P, _I, _P, _P, _I, _I, _I, _I, _I, _I, _P],
     "tfimm_b200_gemm_glu_f32": [_P, _I, _P, _I, _P, _P, _I, _I, _I, _I, _I, _I, _P],
     "tfimm_b200_affine": [_P, _L, _P, _P, _P, _I, _L, _L, _I, _P],
+    # include/tfimm_b200_poolformer.h
+    "tfimm_b200_gn1_partials": [_P, _P, _I, _I, _I, _I, _I, _P],
+    "tfimm_b200_poolformer_mixer": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P],
+    "tfimm_b200_gn1_apply": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _P],
+    # include/tfimm_b200_pit.h
+    "tfimm_b200_pit_attention_bf16": [_P, _P, _I, _I, _I, _I, _F, _P],
+    "tfimm_b200_pit_pool": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P],
+    # include/tfimm_b200_convmixer.h
+    "tfimm_b200_convmixer_dwconv": [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P],
+    # include/tfimm_b200_pvt.h
+    "tfimm_b200_pvt_sr_attention_bf16": [_P, _P, _P, _I, _I, _I, _I, _I, _F, _P],
+    "tfimm_b200_pvt_sr_attention_f32": [_P, _P, _P, _I, _I, _I, _I, _I, _F, _P],
+    "tfimm_b200_pvt_embed_norm": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _P],
+    # include/tfimm_b200_pvt_v2.h
+    "tfimm_b200_pvt_v2_conv_mlp_bf16": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
+    "tfimm_b200_pvt_v2_sr_attention_bf16": [_P, _P, _P, _I, _I, _I, _I, _I, _F, _P],
+    "tfimm_b200_pvt_v2_sr_attention_f32": [_P, _P, _P, _I, _I, _I, _I, _I, _F, _P],
+    # include/tfimm_b200_cait.h
+    "tfimm_b200_cait_talking_heads_bf16": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
+    "tfimm_b200_cait_talking_heads_f32": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
+    "tfimm_b200_cait_class_attention": [_P, _P, _P, _I, _I, _I, _I, _I, _F, _P],
+    "tfimm_b200_cait_add_pos": [_P, _P, _I, _I, _I, _P],
 }
 _SPECIAL = {
     "tfimm_b200_version": ([], _c.c_char_p),
@@ -105,7 +129,7 @@ class KernelLibraryError(RuntimeError):
 
 
 def exported_symbols():
-    """All symbol names the header declares (used by the CPU test-suite)."""
+    """All symbol names the headers declare (used by the CPU test-suite)."""
     return sorted(list(SIGNATURES) + list(_SPECIAL))
 
 

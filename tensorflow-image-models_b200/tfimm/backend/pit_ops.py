@@ -3,46 +3,14 @@ dispatch.
 
 Same conventions as ``tfimm.backend.ops``: torch CUDA tensors in, one library call on the operands' device's current
 stream, counted in ``ops.launch_count`` and bracketed by CUDA events when ``ops.trace`` is set.  Nothing falls back to
-torch ops.  The entry points live in ``libtfimm_b200.so`` but not in ``lib.SIGNATURES``: their ctypes table is here
-and is bound on ``lib.load()``'s handle at first use.
+torch ops.  ``lib.load()`` types their entry points with all the others.
 """
-import ctypes
-
 import torch
 
 from . import lib as _lib
 from . import ops as _ops
 
-_P, _I, _F = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
-
-SIGNATURES = {
-    "tfimm_b200_pit_attention_bf16": [_P, _P, _I, _I, _I, _I, _F, _P],
-    "tfimm_b200_pit_pool": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P],
-}
-# trace family of each entry point (bench.py's roofline rows, tools/ncu_traffic.py)
-TRACE_FAMILY = {name: name[len("tfimm_b200_"):] for name in SIGNATURES}
-
 HEAD_DIMS = (32, 48, 64)
-
-_bound = None
-
-
-def load():
-    """The library handle with this module's entry points typed (once per handle)."""
-    global _bound
-    handle = _lib.load()
-    if _bound is not handle:
-        for name, argtypes in SIGNATURES.items():
-            fn = getattr(handle, name)
-            fn.argtypes = argtypes
-            fn.restype = _I
-        _bound = handle
-    return handle
-
-
-def _call(name, dev, *args, flops=0.0, nbytes=0.0):
-    load()
-    _ops._call(name, dev, *args, flops=flops, nbytes=nbytes, family=TRACE_FAMILY[name])
 
 
 def pool_geometry(H, W):
@@ -57,8 +25,8 @@ def pit_attention_bf16(qkv, B, T, H, dh, scale):
     assert qkv.dtype == torch.bfloat16 and qkv.is_contiguous() and qkv.shape == (B * T, 3 * H * dh), \
         (qkv.dtype, qkv.shape, (B, T, H, dh))
     out = torch.empty((B * T, H * dh), device=qkv.device, dtype=torch.bfloat16)
-    _call("tfimm_b200_pit_attention_bf16", dev, qkv.data_ptr(), out.data_ptr(), B, T, H, dh, float(scale),
-          flops=4.0 * B * H * T * T * dh, nbytes=_ops._nbytes(qkv, out))
+    _ops._call("tfimm_b200_pit_attention_bf16", dev, qkv.data_ptr(), out.data_ptr(), B, T, H, dh, float(scale),
+               flops=4.0 * B * H * T * T * dh, nbytes=_ops._nbytes(qkv, out))
     return out
 
 
@@ -84,9 +52,9 @@ def pit_pool(x, w, bias, B, nb_tokens, H, W, tokens_bf16=False):
     Ho, Wo = pool_geometry(H, W)
     out = torch.empty((B * (nb_tokens + Ho * Wo), 2 * C), device=x.device, dtype=torch.float32)
     tokens = torch.empty((B * nb_tokens, C), device=x.device, dtype=torch.bfloat16) if tokens_bf16 else None
-    _call("tfimm_b200_pit_pool", dev, x.data_ptr(), w.data_ptr(), bias.data_ptr(), out.data_ptr(), _ops._ptr(tokens),
-          B, nb_tokens, H, W, C, flops=2.0 * 9 * B * Ho * Wo * 2 * C,
-          nbytes=pool_nbytes(B, nb_tokens, H, W, C, tokens_bf16))
+    _ops._call("tfimm_b200_pit_pool", dev, x.data_ptr(), w.data_ptr(), bias.data_ptr(), out.data_ptr(),
+               _ops._ptr(tokens), B, nb_tokens, H, W, C, flops=2.0 * 9 * B * Ho * Wo * 2 * C,
+               nbytes=pool_nbytes(B, nb_tokens, H, W, C, tokens_bf16))
     return out, tokens
 
 

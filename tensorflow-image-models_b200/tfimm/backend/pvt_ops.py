@@ -2,47 +2,14 @@
 
 Same conventions as ``tfimm.backend.ops``: torch CUDA tensors in, one library call on the operands' device's current
 stream, counted in ``ops.launch_count`` and bracketed by CUDA events when ``ops.trace`` is set.  Nothing falls back to
-torch ops.  The entry points live in ``libtfimm_b200.so`` but not in ``lib.SIGNATURES``: their ctypes table is here
-and is bound on ``lib.load()``'s handle at first use.
+torch ops.  ``lib.load()`` types their entry points with all the others.
 """
-import ctypes
-
 import torch
 
 from . import lib as _lib
 from . import ops as _ops
 
-_P, _I, _F = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
-
-SIGNATURES = {
-    "tfimm_b200_pvt_sr_attention_bf16": [_P, _P, _P, _I, _I, _I, _I, _I, _F, _P],
-    "tfimm_b200_pvt_sr_attention_f32": [_P, _P, _P, _I, _I, _I, _I, _I, _F, _P],
-    "tfimm_b200_pvt_embed_norm": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _P],
-}
-# trace family of each entry point (bench.py's roofline rows, tools/ncu_traffic.py)
-TRACE_FAMILY = {name: name[len("tfimm_b200_"):] for name in SIGNATURES}
-
 HEAD_DIM = 64
-
-_bound = None
-
-
-def load():
-    """The library handle with this module's entry points typed (once per handle)."""
-    global _bound
-    handle = _lib.load()
-    if _bound is not handle:
-        for name, argtypes in SIGNATURES.items():
-            fn = getattr(handle, name)
-            fn.argtypes = argtypes
-            fn.restype = _I
-        _bound = handle
-    return handle
-
-
-def _call(name, dev, *args, flops=0.0, nbytes=0.0):
-    load()
-    _ops._call(name, dev, *args, flops=flops, nbytes=nbytes, family=TRACE_FAMILY[name])
 
 
 def sr_attention_nbytes(B, N, Nk, H, dh, itemsize):
@@ -55,8 +22,8 @@ def _sr_attention(name, dtype, q, kv, B, N, Nk, H, dh, scale):
     assert q.dtype == kv.dtype == dtype and q.is_contiguous() and kv.is_contiguous(), (q.dtype, kv.dtype)
     assert q.shape == (B * N, H * dh) and kv.shape == (B * Nk, 2 * H * dh), (q.shape, kv.shape, (B, N, Nk, H, dh))
     out = torch.empty((B * N, H * dh), device=q.device, dtype=dtype)
-    _call(name, dev, q.data_ptr(), kv.data_ptr(), out.data_ptr(), B, N, Nk, H, dh, float(scale),
-          flops=4.0 * B * H * N * Nk * dh, nbytes=sr_attention_nbytes(B, N, Nk, H, dh, q.element_size()))
+    _ops._call(name, dev, q.data_ptr(), kv.data_ptr(), out.data_ptr(), B, N, Nk, H, dh, float(scale),
+               flops=4.0 * B * H * N * Nk * dh, nbytes=sr_attention_nbytes(B, N, Nk, H, dh, q.element_size()))
     return out
 
 
@@ -98,7 +65,7 @@ def pvt_embed_norm(tok, gamma, beta, pos, cls, B, P, eps):
     for v in (gamma, beta) if cls is None else (gamma, beta, cls):
         assert v.dtype == torch.float32 and v.is_contiguous() and v.shape == (C,), (v.dtype, v.shape, C)
     out = torch.empty((B * (ntok + P), C), device=tok.device, dtype=torch.float32)
-    _call("tfimm_b200_pvt_embed_norm", dev, tok.data_ptr(), gamma.data_ptr(), beta.data_ptr(), pos.data_ptr(),
-          _ops._ptr(cls), out.data_ptr(), B, P, ntok, C, float(eps), flops=9.0 * B * (P + ntok) * C,
-          nbytes=embed_norm_nbytes(B, P, ntok, C))
+    _ops._call("tfimm_b200_pvt_embed_norm", dev, tok.data_ptr(), gamma.data_ptr(), beta.data_ptr(), pos.data_ptr(),
+               _ops._ptr(cls), out.data_ptr(), B, P, ntok, C, float(eps), flops=9.0 * B * (P + ntok) * C,
+               nbytes=embed_norm_nbytes(B, P, ntok, C))
     return out

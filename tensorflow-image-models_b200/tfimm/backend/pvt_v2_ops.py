@@ -2,26 +2,13 @@
 
 Same conventions as ``tfimm.backend.ops``: torch CUDA tensors in, one library call on the operands' device's current
 stream, counted in ``ops.launch_count`` and bracketed by CUDA events when ``ops.trace`` is set.  Nothing falls back to
-torch ops.  The entry points live in ``libtfimm_b200.so`` but not in ``lib.SIGNATURES``: their ctypes table is here
-and is bound on ``lib.load()``'s handle at first use.
+torch ops.  ``lib.load()`` types their entry points with all the others.
 """
-import ctypes
-
 import torch
 
 from . import lib as _lib
 from . import ops as _ops
 from . import pvt_ops as _pvt_ops
-
-_P, _I, _F = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
-
-SIGNATURES = {
-    "tfimm_b200_pvt_v2_conv_mlp_bf16": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
-    "tfimm_b200_pvt_v2_sr_attention_bf16": [_P, _P, _P, _I, _I, _I, _I, _I, _F, _P],
-    "tfimm_b200_pvt_v2_sr_attention_f32": [_P, _P, _P, _I, _I, _I, _I, _I, _F, _P],
-}
-# trace family of each entry point (bench.py's roofline rows, tools/ncu_traffic.py)
-TRACE_FAMILY = {name: name[len("tfimm_b200_"):] for name in SIGNATURES}
 
 HEAD_DIMS = (32, 64)            # 32: the kernels here; 64: pvt_ops' (PVT v1's)
 CONV_MLP_CHANNELS = (32, 64, 128)
@@ -30,26 +17,6 @@ CONV_MLP_HIDDEN_STEP = 64
 # the three unfused launches on an H100 (profiles/pvt_v2_h100.md: one CTA per SM at 142 registers), so those blocks run
 # the unfused chain.
 CONV_MLP_FUSED_CHANNELS = (32, 64)
-
-_bound = None
-
-
-def load():
-    """The library handle with this module's entry points typed (once per handle)."""
-    global _bound
-    handle = _lib.load()
-    if _bound is not handle:
-        for name, argtypes in SIGNATURES.items():
-            fn = getattr(handle, name)
-            fn.argtypes = argtypes
-            fn.restype = _I
-        _bound = handle
-    return handle
-
-
-def _call(name, dev, *args, flops=0.0, nbytes=0.0):
-    load()
-    _ops._call(name, dev, *args, flops=flops, nbytes=nbytes, family=TRACE_FAMILY[name])
 
 
 # ------------------------------------------------------------------------------------------------------ ConvFFN
@@ -93,10 +60,10 @@ def pvt_v2_conv_mlp_bf16(h, w1, b1, wdw, bdw, w2, b2, residual, B, gh, gw, act, 
     if out is None:
         out = torch.empty_like(residual)
     assert out.dtype == torch.float32 and out.shape == (M, C) and out.is_contiguous()
-    _call("tfimm_b200_pvt_v2_conv_mlp_bf16", dev, h.data_ptr(), w1.data_ptr(), b1.data_ptr(), wdw.data_ptr(),
-          bdw.data_ptr(), w2.data_ptr(), b2.data_ptr(), residual.data_ptr(), out.data_ptr(), B, gh, gw, C, hidden,
-          _ops.act_code(act), flops=2.0 * M * hidden * (2 * C + 9),
-          nbytes=conv_mlp_nbytes(B, gh, gw, C, hidden))
+    _ops._call("tfimm_b200_pvt_v2_conv_mlp_bf16", dev, h.data_ptr(), w1.data_ptr(), b1.data_ptr(), wdw.data_ptr(),
+               bdw.data_ptr(), w2.data_ptr(), b2.data_ptr(), residual.data_ptr(), out.data_ptr(), B, gh, gw, C, hidden,
+               _ops.act_code(act), flops=2.0 * M * hidden * (2 * C + 9),
+               nbytes=conv_mlp_nbytes(B, gh, gw, C, hidden))
     return out
 
 
@@ -130,8 +97,8 @@ def _sr_attention(name, dtype, q, kv, B, N, Nk, H, dh, scale):
     assert q.dtype == kv.dtype == dtype and q.is_contiguous() and kv.is_contiguous(), (q.dtype, kv.dtype)
     assert q.shape == (B * N, H * dh) and kv.shape == (B * Nk, 2 * H * dh), (q.shape, kv.shape, (B, N, Nk, H, dh))
     out = torch.empty((B * N, H * dh), device=q.device, dtype=dtype)
-    _call(name, dev, q.data_ptr(), kv.data_ptr(), out.data_ptr(), B, N, Nk, H, dh, float(scale),
-          flops=4.0 * B * H * N * Nk * dh, nbytes=_pvt_ops.sr_attention_nbytes(B, N, Nk, H, dh, q.element_size()))
+    _ops._call(name, dev, q.data_ptr(), kv.data_ptr(), out.data_ptr(), B, N, Nk, H, dh, float(scale),
+               flops=4.0 * B * H * N * Nk * dh, nbytes=_pvt_ops.sr_attention_nbytes(B, N, Nk, H, dh, q.element_size()))
     return out
 
 

@@ -1,11 +1,10 @@
-"""CPU tests of the drop-in boundary: registry, factory, preprocessing, weight transfer, cache, C ABI exports.
+"""CPU tests of the drop-in boundary: registry, factory, preprocessing, weight transfer, cache.
 
 They mirror the reference's tests/models/test_factory.py, tests/utils/test_cache.py and tests/utils/test_etc.py
 for everything that does not need a forward pass (forward parity lives in the -m gpu tests).
 """
 import json
 import logging
-import re
 import subprocess
 from pathlib import Path
 
@@ -212,34 +211,6 @@ def test_etc_helpers():
     assert to_2tuple(3) == (3, 3) and to_2tuple((1, 2, 3)) == (1, 2)
     assert [make_divisible(v, 8) for v in (32 * 1.4, 16 * 1.4, 24 * 1.4, 1280 * 1.4, 10, 3)] == [48, 24, 32, 1792, 16, 8]
     assert make_divisible(2048 * 0.0625, 8, round_limit=0.0) == 128
-
-
-def test_c_abi_library_exports_every_declared_symbol():
-    """The .so loads without a GPU and exports exactly what include/tfimm_b200.h declares."""
-    from tfimm.backend import lib
-
-    handle = lib.load()
-    header = (ROOT / "include" / "tfimm_b200.h").read_text()
-    declared = set(re.findall(r"\b(tfimm_b200_[a-z0-9_]+)\s*\(", header))
-    assert declared == set(lib.exported_symbols()), declared ^ set(lib.exported_symbols())
-    nm = subprocess.run(["nm", "-D", "--defined-only", str(lib.LIB_PATH)], capture_output=True, text=True).stdout
-    exported = set(re.findall(r"\sT\s+(tfimm_b200_[a-z0-9_]+)", nm))
-    assert declared <= exported, declared - exported
-    assert handle.tfimm_b200_version().decode().startswith("tfimm_b200")
-    # arity of every binding matches the header's parameter list
-    for name, argtypes in lib.SIGNATURES.items():
-        m = re.search(name + r"\s*\(([^;]*?)\)\s*;", header, re.S)
-        assert m, name
-        params = [p.strip() for p in m.group(1).split(",") if p.strip() and p.strip() != "void"]
-        assert len(params) == len(argtypes), (name, len(params), len(argtypes))
-        # ... and so does the kind of every parameter (pointer / int / long / float): a float passed as int, or a
-        # 64-bit stride passed as int, would be silent garbage through ctypes
-        import ctypes
-
-        for p, ct in zip(params, argtypes):
-            want = ctypes.c_void_p if "*" in p else ctypes.c_float if p.startswith("float") else \
-                ctypes.c_long if p.startswith("long") else ctypes.c_int
-            assert ct is want, (name, p, ct)
 
 
 def test_every_kernel_of_the_library_belongs_to_a_bench_family():

@@ -185,7 +185,7 @@ def _launch(name, qkv, B, out=None):
     if name.startswith("pit"):
         if out is None:
             return pit_ops.pit_attention_bf16(qkv, B, N, H, dh, scale)
-        return pit_ops.load().tfimm_b200_pit_attention_bf16(qkv.data_ptr(), out.data_ptr(), B, N, H, dh, scale, None)
+        return lib.load().tfimm_b200_pit_attention_bf16(qkv.data_ptr(), out.data_ptr(), B, N, H, dh, scale, None)
     entry = "tfimm_b200_attention_tf32" if name == "attention_tf32" else "tfimm_b200_attention_bf16"
     with _tf32_mode():
         if out is None:

@@ -1,10 +1,8 @@
-"""CaiT family on CPU: opt-in registration (and the registry left as it was found), the C entry points and their ctypes
-table, the attention dispatch, the refusals, the host orchestration on the float64 statements, the float32 shadow
-rehearsal and seeded defects."""
-import ctypes
+"""CaiT family on CPU: opt-in registration (and the registry left as it was found), the C entry points' argument checks,
+the attention dispatch, the refusals, the host orchestration on the float64 statements, the float32 shadow rehearsal and
+seeded defects."""
 import dataclasses
 import math
-import re
 import subprocess
 import sys
 from pathlib import Path
@@ -67,31 +65,13 @@ def test_param_specs_initial_values(cait):
 
 
 PREFIX = "tfimm_b200_"
-ZERO_CALL = {
-    "cait_talking_heads_bf16": (1, "cait_talking_heads_bf16: bad shape B=0 N=0 H=0"),
-    "cait_talking_heads_f32": (1, "cait_talking_heads_f32: bad shape B=0 N=0 H=0"),
-    "cait_class_attention": (1, "cait_class_attention: bad shape B=0 T=0 H=0"),
-    "cait_add_pos": (1, "cait_add_pos: need B, N > 0 and D % 4 == 0 (B=0 N=0 D=0)"),
-}
-
-
-def test_entry_points_reject_all_zero_arguments_with_their_own_message():
-    from tfimm.backend import cait_ops
-
-    handle = cait_ops.load()
-    assert {PREFIX + n for n in ZERO_CALL} == set(cait_ops.SIGNATURES)
-    got = {}
-    for name, argtypes in cait_ops.SIGNATURES.items():
-        args = [None if t is ctypes.c_void_p else 0.0 if t is ctypes.c_float else 0 for t in argtypes]
-        got[name[len(PREFIX):]] = (getattr(handle, name)(*args), handle.tfimm_b200_last_error().decode())
-    assert got == ZERO_CALL
 
 
 def test_entry_point_argument_checks_past_the_shape():
     """Shapes without an instantiation, misaligned or missing pointers are refused before any CUDA call."""
-    from tfimm.backend import cait_ops, lib
+    from tfimm.backend import lib
 
-    h = cait_ops.load()
+    h = lib.load()
     assert h.tfimm_b200_cait_talking_heads_bf16(16, 16, 16, 16, 16, 16, 2, 197, 12, 64, None) == 1
     assert "head_dim 48 and H in {4, 6, 8, 16} (got H=12 dh=64)" in h.tfimm_b200_last_error().decode()
     assert h.tfimm_b200_cait_talking_heads_bf16(16, 16, 16, 16, 16, 16, 2, 197, 5, 48, None) == 1
@@ -110,27 +90,9 @@ def test_entry_point_argument_checks_past_the_shape():
     assert h.tfimm_b200_cait_add_pos(16, 16, 2, 196, 190, None) == 1
 
 
-def test_header_declares_the_ctypes_table():
-    from tfimm.backend import cait_ops, lib
-
-    header = (ROOT / "include" / "tfimm_b200_cait.h").read_text()
-    assert set(re.findall(r"^int (tfimm_b200_[a-z0-9_]+)\(", header, re.M)) == set(cait_ops.SIGNATURES)
-    core = (ROOT / "include" / "tfimm_b200.h").read_text()
-    nm = subprocess.run(["nm", "-D", "--defined-only", str(lib.LIB_PATH)], capture_output=True, text=True).stdout
-    for name, argtypes in cait_ops.SIGNATURES.items():
-        assert name not in core and name not in lib.SIGNATURES and re.search(r"\sT\s+" + name + r"\b", nm)
-        params = [p.strip() for p in re.search(name + r"\s*\(([^;]*?)\)\s*;", header, re.S).group(1).split(",")]
-        assert len(params) == len(argtypes), name
-        for p, ct in zip(params, argtypes):
-            want = ctypes.c_void_p if "*" in p else ctypes.c_float if p.startswith("float") else ctypes.c_int
-            assert ct is want, (name, p, ct)
-
-
 def test_trace_family_names_and_counts():
     from tfimm.backend import cait_ops, ops
 
-    assert cait_ops.TRACE_FAMILY == {n: n[len(PREFIX):] for n in cait_ops.SIGNATURES}
-    assert not set(cait_ops.SIGNATURES) & set(ops.TRACE_FAMILY)
     sys.path.insert(0, str(ROOT / "tools"))
     import ncu_traffic
 
@@ -139,7 +101,7 @@ def test_trace_family_names_and_counts():
                         ("cait_talking_heads_f32_kernel<6>(const float *)", "cait_talking_heads_f32"),
                         ("cait_class_attn_kernel<float, 48>(const float *)", "cait_class_attention"),
                         ("cait_add_pos_kernel(float4 *)", "cait_add_pos")):
-        assert ncu_traffic.family_of(ns + kernel) == fam == cait_ops.TRACE_FAMILY[PREFIX + fam]
+        assert ncu_traffic.family_of(ns + kernel) == fam == ops.TRACE_FAMILY[PREFIX + fam]
     # q k^T twice and P' V once (2 H dh FMA each per pair), the two H x H mixes (pre-mix twice)
     assert cait_ops.talking_heads_flops(2, 196, 4, 48) == 2.0 * 2 * 196 * 196 * (3 * 192 + 3 * 16)
 

@@ -134,7 +134,7 @@ def test_guard_regions_untouched():
     """Outputs written into the middle of larger buffers: the guard cells on both sides keep their pattern."""
     from tfimm.backend import cait_ops, lib
 
-    h = cait_ops.load()
+    h = lib.load()
     G = 4096
     pattern = -1232.0   # exact in bf16
 

@@ -127,9 +127,8 @@ def test_guard_regions_untouched(out):
     n = B * H * W * C
     buf = torch.full((n + 2 * G,), 777.0, device="cuda").to(out)
     y = buf[G:G + n]
-    convmixer_ops.load()
     ops._call("tfimm_b200_convmixer_dwconv", a.device, a.data_ptr(), *(t.data_ptr() for t in p), y.data_ptr(),
-              ops._code(y), B, H, W, C, k, ops.act_code("gelu"), family="convmixer_dwconv")
+              ops._code(y), B, H, W, C, k, ops.act_code("gelu"))
     torch.cuda.synchronize()
     guard = torch.cat((buf[:G], buf[-G:]))
     assert torch.equal(guard, torch.full_like(guard, 777.0).to(torch.float32).to(out))

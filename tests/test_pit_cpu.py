@@ -1,10 +1,8 @@
-"""PiT family on CPU: opt-in registration (and the registry left as it was found), the C entry points and their ctypes
-table, the attention dispatch, the host orchestration on the float64 statements, the float32 shadow rehearsal and
-seeded defects."""
-import ctypes
+"""PiT family on CPU: opt-in registration (and the registry left as it was found), the C entry points' argument checks,
+the attention dispatch, the host orchestration on the float64 statements, the float32 shadow rehearsal and seeded
+defects."""
 import dataclasses
 import importlib
-import re
 import subprocess
 import sys
 from copy import deepcopy
@@ -56,30 +54,14 @@ def test_registration_on_import(pit):
 
 
 PREFIX = "tfimm_b200_"
-ZERO_CALL = {
-    "pit_attention_bf16": (1, "pit_attention_bf16: bad shape B=0 T=0 H=0"),
-    "pit_pool": (1, "pit_pool: need B, H, W > 0, C % 4 == 0 and nb_tokens >= 0 (B=0 H=0 W=0 C=0 nb_tokens=0)"),
-}
-
-
-def test_entry_points_reject_all_zero_arguments_with_their_own_message():
-    from tfimm.backend import pit_ops
-
-    handle = pit_ops.load()
-    assert {PREFIX + n for n in ZERO_CALL} == set(pit_ops.SIGNATURES)
-    got = {}
-    for name, argtypes in pit_ops.SIGNATURES.items():
-        args = [None if t is ctypes.c_void_p else 0.0 if t is ctypes.c_float else 0 for t in argtypes]
-        got[name[len(PREFIX):]] = (getattr(handle, name)(*args), handle.tfimm_b200_last_error().decode())
-    assert got == ZERO_CALL
 
 
 def test_entry_point_argument_checks_past_the_shape():
     """Head dims other than 32 / 48 / 64, misaligned pointers and a token copy without token rows are refused before
     any CUDA call."""
-    from tfimm.backend import pit_ops
+    from tfimm.backend import lib, pit_ops
 
-    h = pit_ops.load()
+    h = lib.load()
     assert h.tfimm_b200_pit_attention_bf16(16, 16, 2, 197, 4, 40, 0.1, None) == 1
     assert "head_dim must be 32, 48 or 64 (got 40)" in h.tfimm_b200_last_error().decode()
     assert h.tfimm_b200_pit_attention_bf16(16, 24, 2, 197, 4, 32, 0.1, None) == 1
@@ -92,36 +74,16 @@ def test_entry_point_argument_checks_past_the_shape():
     assert pit_ops.pool_geometry(1, 1) == (1, 1) and pit_ops.pool_geometry(6, 5) == (3, 3)
 
 
-def test_header_declares_the_ctypes_table():
-    """include/tfimm_b200_pit.h declares exactly the two entry points, each parameter of the kind the ctypes table
-    passes, and the library exports them; the core header does not name them."""
-    from tfimm.backend import lib, pit_ops
-
-    header = (ROOT / "include" / "tfimm_b200_pit.h").read_text()
-    assert set(re.findall(r"^int (tfimm_b200_[a-z0-9_]+)\(", header, re.M)) == set(pit_ops.SIGNATURES)
-    core = (ROOT / "include" / "tfimm_b200.h").read_text()
-    nm = subprocess.run(["nm", "-D", "--defined-only", str(lib.LIB_PATH)], capture_output=True, text=True).stdout
-    for name, argtypes in pit_ops.SIGNATURES.items():
-        assert name not in core and name not in lib.SIGNATURES and re.search(r"\sT\s+" + name + r"\b", nm)
-        params = [p.strip() for p in re.search(name + r"\s*\(([^;]*?)\)\s*;", header, re.S).group(1).split(",")]
-        assert len(params) == len(argtypes), name
-        for p, ct in zip(params, argtypes):
-            want = ctypes.c_void_p if "*" in p else ctypes.c_float if p.startswith("float") else \
-                ctypes.c_long if p.startswith("long") else ctypes.c_int
-            assert ct is want, (name, p, ct)
-
-
 def test_trace_family_names():
-    from tfimm.backend import ops, pit_ops
+    from tfimm.backend import ops
 
-    assert pit_ops.TRACE_FAMILY == {n: n[len(PREFIX):] for n in pit_ops.SIGNATURES}
-    assert not set(pit_ops.SIGNATURES) & set(ops.TRACE_FAMILY)
     sys.path.insert(0, str(ROOT / "tools"))
     import ncu_traffic
 
     assert ncu_traffic.family_of("void tfimm::(anonymous namespace)::pit_attention_bf16_kernel<48>(const __nv_bfloat16 *)") \
-        == "pit_attention_bf16"
-    assert ncu_traffic.family_of("tfimm::(anonymous namespace)::pit_pool_kernel(const float *)") == "pit_pool"
+        == "pit_attention_bf16" == ops.TRACE_FAMILY[PREFIX + "pit_attention_bf16"]
+    assert ncu_traffic.family_of("tfimm::(anonymous namespace)::pit_pool_kernel(const float *)") == "pit_pool" == \
+        ops.TRACE_FAMILY[PREFIX + "pit_pool"]
 
 
 def test_byte_counts():

@@ -130,9 +130,9 @@ def test_pool_against_float64(case):
 def test_guard_regions_untouched():
     """Outputs written into the middle of larger buffers: the guard cells on both sides keep their pattern, and the
     token rows of the pooled stream (the token Dense's) are not written."""
-    from tfimm.backend import pit_ops
+    from tfimm.backend import lib, pit_ops
 
-    h = pit_ops.load()
+    h = lib.load()
     G = 4096   # guard elements on each side (16-byte multiples)
     pattern = -1232.0   # exact in bf16
 

@@ -1,8 +1,6 @@
-"""PoolFormer family on CPU: opt-in registration (and the registry left as it was found), the C entry points and their
-ctypes table, the host orchestration on the float64 statements, the float32 shadow rehearsal and seeded defects."""
-import ctypes
+"""PoolFormer family on CPU: opt-in registration (and the registry left as it was found), the C entry points' argument
+checks, the host orchestration on the float64 statements, the float32 shadow rehearsal and seeded defects."""
 import importlib
-import re
 import subprocess
 import sys
 from copy import deepcopy
@@ -54,30 +52,13 @@ def test_registration_on_import(poolformer):
 
 
 PREFIX = "tfimm_b200_"
-ZERO_CALL = {
-    "gn1_partials": (1, "gn1_partials: need B, H, W > 0 and C % 4 == 0 (B=0 H=0 W=0 C=0)"),
-    "poolformer_mixer": (1, "poolformer_mixer: need B, H, W > 0 and C % 4 == 0 (B=0 H=0 W=0 C=0)"),
-    "gn1_apply": (1, "gn1_apply: need B, H, W > 0 and C % 4 == 0 (B=0 H=0 W=0 C=0)"),
-}
-
-
-def test_entry_points_reject_all_zero_arguments_with_their_own_message():
-    from tfimm.backend import poolformer_ops
-
-    handle = poolformer_ops.load()
-    assert {PREFIX + n for n in ZERO_CALL} == set(poolformer_ops.SIGNATURES)
-    got = {}
-    for name, argtypes in poolformer_ops.SIGNATURES.items():
-        args = [None if t is ctypes.c_void_p else 0.0 if t is ctypes.c_float else 0 for t in argtypes]
-        got[name[len(PREFIX):]] = (getattr(handle, name)(*args), handle.tfimm_b200_last_error().decode())
-    assert got == ZERO_CALL
 
 
 def test_entry_point_argument_checks_past_the_shape():
     """A wrong chunking and an in-place mixer are refused before any CUDA call."""
-    from tfimm.backend import poolformer_ops
+    from tfimm.backend import lib, poolformer_ops
 
-    h = poolformer_ops.load()
+    h = lib.load()
     assert h.tfimm_b200_gn1_partials(16, 16, 1, 56, 56, 64, 3, None) == 1
     assert "splits 3, the chunking of H*W*C=200704 gives 49" in h.tfimm_b200_last_error().decode()
     assert h.tfimm_b200_poolformer_mixer(16, 16, 16, 16, 16, 32, 1, 7, 7, 64, 1, 1e-5, None) == 1
@@ -87,36 +68,16 @@ def test_entry_point_argument_checks_past_the_shape():
     assert poolformer_ops.splits(56, 56, 64) == 49 and poolformer_ops.splits(1, 1, 512) == 1
 
 
-def test_header_declares_the_ctypes_table():
-    """include/tfimm_b200_poolformer.h declares exactly the three entry points, each parameter of the kind the ctypes
-    table passes, and the library exports them; the core header does not name them."""
-    from tfimm.backend import lib, poolformer_ops
-
-    header = (ROOT / "include" / "tfimm_b200_poolformer.h").read_text()
-    assert set(re.findall(r"^int (tfimm_b200_[a-z0-9_]+)\(", header, re.M)) == set(poolformer_ops.SIGNATURES)
-    core = (ROOT / "include" / "tfimm_b200.h").read_text()
-    nm = subprocess.run(["nm", "-D", "--defined-only", str(lib.LIB_PATH)], capture_output=True, text=True).stdout
-    for name, argtypes in poolformer_ops.SIGNATURES.items():
-        assert name not in core and name not in lib.SIGNATURES and re.search(r"\sT\s+" + name + r"\b", nm)
-        params = [p.strip() for p in re.search(name + r"\s*\(([^;]*?)\)\s*;", header, re.S).group(1).split(",")]
-        assert len(params) == len(argtypes), name
-        for p, ct in zip(params, argtypes):
-            want = ctypes.c_void_p if "*" in p else ctypes.c_float if p.startswith("float") else \
-                ctypes.c_long if p.startswith("long") else ctypes.c_int
-            assert ct is want, (name, p, ct)
-
-
 def test_trace_family_names():
-    from tfimm.backend import ops, poolformer_ops
+    from tfimm.backend import ops
 
-    assert poolformer_ops.TRACE_FAMILY == {n: n[len(PREFIX):] for n in poolformer_ops.SIGNATURES}
-    assert not set(poolformer_ops.SIGNATURES) & set(ops.TRACE_FAMILY)
     sys.path.insert(0, str(ROOT / "tools"))
     import ncu_traffic
 
     for kernel in ("gn1_partials_kernel", "poolformer_mixer_kernel", "gn1_apply_kernel<float>"):
-        assert ncu_traffic.family_of(f"tfimm::(anonymous namespace)::{kernel}(const float *)") == \
-            kernel.split("_kernel")[0]
+        fam = kernel.split("_kernel")[0]
+        assert ncu_traffic.family_of(f"tfimm::(anonymous namespace)::{kernel}(const float *)") == fam == \
+            ops.TRACE_FAMILY[PREFIX + fam]
 
 
 def test_byte_counts():

@@ -129,11 +129,11 @@ def test_guard_regions_untouched():
     obuf, out = guarded(B * N, torch.float32)
     qbuf, p2 = guarded(B * S * 3, torch.float32)
     ybuf, y = guarded(B * N, torch.bfloat16)
-    poolformer_ops._call("tfimm_b200_gn1_partials", dev, x.data_ptr(), p.data_ptr(), B, H, W, C, S)
-    poolformer_ops._call("tfimm_b200_poolformer_mixer", dev, x.data_ptr(), p.data_ptr(), gamma.data_ptr(),
-                         ls1.data_ptr(), out.data_ptr(), p2.data_ptr(), B, H, W, C, S, 1e-5)
-    poolformer_ops._call("tfimm_b200_gn1_apply", dev, out.data_ptr(), p2.data_ptr(), gamma.data_ptr(),
-                         beta.data_ptr(), y.data_ptr(), ops.BF16, B, H, W, C, S, 1e-5)
+    ops._call("tfimm_b200_gn1_partials", dev, x.data_ptr(), p.data_ptr(), B, H, W, C, S)
+    ops._call("tfimm_b200_poolformer_mixer", dev, x.data_ptr(), p.data_ptr(), gamma.data_ptr(), ls1.data_ptr(),
+              out.data_ptr(), p2.data_ptr(), B, H, W, C, S, 1e-5)
+    ops._call("tfimm_b200_gn1_apply", dev, out.data_ptr(), p2.data_ptr(), gamma.data_ptr(), beta.data_ptr(),
+              y.data_ptr(), ops.BF16, B, H, W, C, S, 1e-5)
     torch.cuda.synchronize()
     for buf in (pbuf, obuf, qbuf, ybuf):
         guard = torch.cat((buf[:G], buf[-G:]))

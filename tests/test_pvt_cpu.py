@@ -1,9 +1,7 @@
-"""PVT family on CPU: opt-in registration (and the registry left as it was found), the C entry points and their ctypes
-table, the attention dispatch, refusals, the host orchestration on the float64 statements, the statements against the
-existing attention statement, the float32 shadow rehearsal and seeded defects."""
-import ctypes
+"""PVT family on CPU: opt-in registration (and the registry left as it was found), the C entry points' argument checks,
+the attention dispatch, refusals, the host orchestration on the float64 statements, the statements against the existing
+attention statement, the float32 shadow rehearsal and seeded defects."""
 import dataclasses
-import re
 import subprocess
 import sys
 from pathlib import Path
@@ -45,32 +43,14 @@ def test_registration_on_import(pvt):
 
 
 PREFIX = "tfimm_b200_"
-ZERO_CALL = {
-    "pvt_sr_attention_bf16": (1, "pvt_sr_attention_bf16: bad shape B=0 N=0 Nk=0 H=0"),
-    "pvt_sr_attention_f32": (1, "pvt_sr_attention_f32: bad shape B=0 N=0 Nk=0 H=0"),
-    "pvt_embed_norm": (1, "pvt_embed_norm: need B, P > 0, ntok 0 or 1, C % 4 == 0 and C <= 1024 "
-                          "(B=0 P=0 ntok=0 C=0)"),
-}
-
-
-def test_entry_points_reject_all_zero_arguments_with_their_own_message():
-    from tfimm.backend import pvt_ops
-
-    handle = pvt_ops.load()
-    assert {PREFIX + n for n in ZERO_CALL} == set(pvt_ops.SIGNATURES)
-    got = {}
-    for name, argtypes in pvt_ops.SIGNATURES.items():
-        args = [None if t is ctypes.c_void_p else 0.0 if t is ctypes.c_float else 0 for t in argtypes]
-        got[name[len(PREFIX):]] = (getattr(handle, name)(*args), handle.tfimm_b200_last_error().decode())
-    assert got == ZERO_CALL
 
 
 def test_entry_point_argument_checks_past_the_shape():
     """Head dims other than 64, too many images or heads, misaligned pointers and a class row without cls are refused
     before any CUDA call."""
-    from tfimm.backend import pvt_ops
+    from tfimm.backend import lib
 
-    h = pvt_ops.load()
+    h = lib.load()
     assert h.tfimm_b200_pvt_sr_attention_bf16(16, 16, 16, 2, 197, 49, 4, 32, 0.1, None) == 1
     assert "head_dim must be 64 (got 32)" in h.tfimm_b200_last_error().decode()
     assert h.tfimm_b200_pvt_sr_attention_bf16(16, 16, 16, 65536, 197, 49, 1, 64, 0.1, None) == 1
@@ -87,37 +67,17 @@ def test_entry_point_argument_checks_past_the_shape():
     assert h.tfimm_b200_pvt_embed_norm(16, 16, 16, 16, None, 16, 2, 49, 2, 64, 1e-5, None) == 1
 
 
-def test_header_declares_the_ctypes_table():
-    """include/tfimm_b200_pvt.h declares exactly the three entry points, each parameter of the kind the ctypes table
-    passes, and the library exports them; the core header does not name them."""
-    from tfimm.backend import lib, pvt_ops
-
-    header = (ROOT / "include" / "tfimm_b200_pvt.h").read_text()
-    assert set(re.findall(r"^int (tfimm_b200_[a-z0-9_]+)\(", header, re.M)) == set(pvt_ops.SIGNATURES)
-    core = (ROOT / "include" / "tfimm_b200.h").read_text()
-    nm = subprocess.run(["nm", "-D", "--defined-only", str(lib.LIB_PATH)], capture_output=True, text=True).stdout
-    for name, argtypes in pvt_ops.SIGNATURES.items():
-        assert name not in core and name not in lib.SIGNATURES and re.search(r"\sT\s+" + name + r"\b", nm)
-        params = [p.strip() for p in re.search(name + r"\s*\(([^;]*?)\)\s*;", header, re.S).group(1).split(",")]
-        assert len(params) == len(argtypes), name
-        for p, ct in zip(params, argtypes):
-            want = ctypes.c_void_p if "*" in p else ctypes.c_float if p.startswith("float") else \
-                ctypes.c_long if p.startswith("long") else ctypes.c_int
-            assert ct is want, (name, p, ct)
-
-
 def test_trace_family_names():
-    from tfimm.backend import ops, pit_ops, pvt_ops
+    from tfimm.backend import ops
 
-    assert pvt_ops.TRACE_FAMILY == {n: n[len(PREFIX):] for n in pvt_ops.SIGNATURES}
-    assert not set(pvt_ops.SIGNATURES) & (set(ops.TRACE_FAMILY) | set(pit_ops.SIGNATURES))
     sys.path.insert(0, str(ROOT / "tools"))
     import ncu_traffic
 
     ns = "tfimm::(anonymous namespace)::"
-    assert ncu_traffic.family_of(f"{ns}pvt_sr_attention_bf16_kernel(const __nv_bfloat16 *)") == "pvt_sr_attention_bf16"
-    assert ncu_traffic.family_of(f"{ns}pvt_sr_attention_f32_kernel(const float *)") == "pvt_sr_attention_f32"
-    assert ncu_traffic.family_of(f"void {ns}pvt_embed_norm_kernel<4>(const float *)") == "pvt_embed_norm"
+    for kernel, fam in ((f"{ns}pvt_sr_attention_bf16_kernel(const __nv_bfloat16 *)", "pvt_sr_attention_bf16"),
+                        (f"{ns}pvt_sr_attention_f32_kernel(const float *)", "pvt_sr_attention_f32"),
+                        (f"void {ns}pvt_embed_norm_kernel<4>(const float *)", "pvt_embed_norm")):
+        assert ncu_traffic.family_of(kernel) == fam == ops.TRACE_FAMILY[PREFIX + fam]
 
 
 def test_byte_counts():

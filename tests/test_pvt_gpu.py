@@ -135,9 +135,9 @@ def _buffer(n, dtype):
 def test_outputs_stay_inside_their_buffers():
     """Through the C entry points, into the middle of a canary buffer: nothing outside the output is written, the
     output holds no canary and no NaN, and it equals the launcher's."""
-    from tfimm.backend import pvt_ops
+    from tfimm.backend import lib, pvt_ops
 
-    h = pvt_ops.load()
+    h = lib.load()
     for dtype, fn in ((torch.bfloat16, h.tfimm_b200_pvt_sr_attention_bf16),
                       (torch.float32, h.tfimm_b200_pvt_sr_attention_f32)):
         for B, N, Nk, H in ((3, 131, 49, 2), (2, 65, 257, 1)):

@@ -121,23 +121,23 @@ G = 4096
 
 
 def test_outputs_stay_inside_their_buffers():
-    from tfimm.backend import pvt_v2_ops
+    from tfimm.backend import lib, pvt_v2_ops
 
-    lib = pvt_v2_ops.load()
+    handle = lib.load()
     for B, gh, gw, C, hidden in ((2, 13, 17, 64, 128), (1, 1, 7, 32, 64), (2, 9, 33, 128, 64)):
         h, w1, b1, wdw, bdw, w2, b2, res = conv_inputs(B, gh, gw, C, hidden, seed=9)
         buf = torch.full((G + res.numel() + G,), -12345.0, device="cuda")
         out = buf[G:G + res.numel()]
-        assert lib.tfimm_b200_pvt_v2_conv_mlp_bf16(h.data_ptr(), w1.data_ptr(), b1.data_ptr(), wdw.data_ptr(),
-                                                   bdw.data_ptr(), w2.data_ptr(), b2.data_ptr(), res.data_ptr(),
-                                                   out.data_ptr(), B, gh, gw, C, hidden, 1, None) == 0
+        assert handle.tfimm_b200_pvt_v2_conv_mlp_bf16(h.data_ptr(), w1.data_ptr(), b1.data_ptr(), wdw.data_ptr(),
+                                                      bdw.data_ptr(), w2.data_ptr(), b2.data_ptr(), res.data_ptr(),
+                                                      out.data_ptr(), B, gh, gw, C, hidden, 1, None) == 0
         torch.cuda.synchronize()
         assert (buf[:G] == -12345.0).all() and (buf[-G:] == -12345.0).all()
         assert not (out == -12345.0).any() and not out.isnan().any()
         assert torch.equal(out.view(-1, C), pvt_v2_ops.pvt_v2_conv_mlp_bf16(h, w1, b1, wdw, bdw, w2, b2, res, B, gh,
                                                                            gw, "gelu"))
-    for dtype, fn in ((torch.bfloat16, lib.tfimm_b200_pvt_v2_sr_attention_bf16),
-                      (torch.float32, lib.tfimm_b200_pvt_v2_sr_attention_f32)):
+    for dtype, fn in ((torch.bfloat16, handle.tfimm_b200_pvt_v2_sr_attention_bf16),
+                      (torch.float32, handle.tfimm_b200_pvt_v2_sr_attention_f32)):
         B, N, Nk, H = 3, 131, 49, 2
         q = torch.randn((B * N, H * DH)).to(dtype).cuda()
         kv = torch.randn((B * Nk, 2 * H * DH)).to(dtype).cuda()
@@ -150,16 +150,16 @@ def test_outputs_stay_inside_their_buffers():
 
 
 def test_conv_mlp_refuses_other_shapes():
-    from tfimm.backend import pvt_v2_ops
+    from tfimm.backend import lib, pvt_v2_ops
 
     h, w1, b1, wdw, bdw, w2, b2, res = conv_inputs(1, 4, 4, 64, 128, seed=1)
     with pytest.raises(ValueError):
         pvt_v2_ops.pvt_v2_conv_mlp_bf16(h, w1[:96], b1[:96], wdw[:, :96], bdw[:96], w2[:, :96].contiguous(), b2, res,
                                         1, 4, 4, "gelu")
-    lib = pvt_v2_ops.load()
-    assert lib.tfimm_b200_pvt_v2_conv_mlp_bf16(h.data_ptr(), w1.data_ptr(), b1.data_ptr(), wdw.data_ptr(),
-                                               bdw.data_ptr(), w2.data_ptr(), b2.data_ptr(), res.data_ptr(),
-                                               res.data_ptr(), 1, 4, 4, 96, 128, 1, None) != 0
+    handle = lib.load()
+    assert handle.tfimm_b200_pvt_v2_conv_mlp_bf16(h.data_ptr(), w1.data_ptr(), b1.data_ptr(), wdw.data_ptr(),
+                                                  bdw.data_ptr(), w2.data_ptr(), b2.data_ptr(), res.data_ptr(),
+                                                  res.data_ptr(), 1, 4, 4, 96, 128, 1, None) != 0
 
 
 def test_determinism_and_batch_independence():
